@@ -48,7 +48,9 @@ struct GemmArgs {
 //   1  64 x __half                                                          128 B
 //   2  "p24": 64 x u16 (bits 31..16 of the float) then 64 x u8 (bits 15..8)  192 B.  The decoder rebuilds a float
 //      with ONE byte permute per element by repeating the third byte as the fourth (value bits = hi16:lo8:lo8), and
-//      the encoder picks the nearest value of that form: 16 mantissa bits, relative error <= 2^-17.
+//      the encoder picks the nearest value of that form.  Within a binade those values are 257 ulps apart (1 ulp where
+//      the low byte wraps from 0xFF to 0x00), so the nearest one is at most 128 ulps away: relative error < 2^-16.
+//      Neighbouring values are an odd number of ulps apart, so there are no ties.
 __host__ __device__ __forceinline__ int kv_row_bytes(int kv_fmt) { return kv_fmt == 0 ? 256 : (kv_fmt == 1 ? 128 : 192); }
 
 __device__ __forceinline__ long long kv_dest(int m, int c, int rows_per_b, int cap, int H, int pos, int kv_fmt, int& d) {
@@ -58,7 +60,8 @@ __device__ __forceinline__ long long kv_dest(int m, int c, int rows_per_b, int c
   return ((((long long)b * 2 + which) * H + h) * cap + t) * kv_row_bytes(kv_fmt);
 }
 
-// the 24 stored bits (hi16 << 8 | lo8) of the p24 value nearest to x
+// the 24 stored bits (hi16 << 8 | lo8) of the p24 value nearest to x: the candidates are the codes t = bits >> 8 and
+// t +- 1 (t - 1 only while it keeps the sign); on equal distance the earlier of t, t + 1, t - 1 would be kept
 __device__ __forceinline__ uint32_t p24_encode(float x) {
   const uint32_t bits = __float_as_uint(x);
   const uint32_t t = bits >> 8;

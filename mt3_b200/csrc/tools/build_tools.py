@@ -1,23 +1,38 @@
-"""Builds the standalone kernel bring-up binaries next to this file (sm_90a)."""
+"""Builds the standalone kernel bring-up binaries and the test-only kernel harness library
+(libmt3kernels.so, loaded by tests/test_kernel_parity.py) next to this file (sm_90a).  A re-run is
+a no-op when every output is newer than the kernel sources."""
 import os
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TOOLS = ["gemm_tc_test", "attn_tc_test"]
+HARNESS = os.path.join(HERE, "libmt3kernels.so")
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr"]
+
+
+def _stale(out, src):
+    csrc = os.path.join(HERE, "..")
+    deps = [src, os.path.abspath(__file__)] + [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cuh", ".cu"))]
+    return not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(d) for d in deps)
+
+
+def harness_stale():
+    return _stale(HARNESS, os.path.join(HERE, "kernel_harness.cu"))
 
 
 def main():
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     for t in TOOLS:
         src, out = os.path.join(HERE, t + ".cu"), os.path.join(HERE, t)
-        deps = [src] + [os.path.join(HERE, "..", f) for f in os.listdir(os.path.join(HERE, "..")) if f.endswith((".cuh", ".cu"))]
-        if os.path.exists(out) and os.path.getmtime(out) >= max(os.path.getmtime(d) for d in deps):
+        if not _stale(out, src):
             continue
-        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-               "--expt-relaxed-constexpr", "-o", out, src]
-        subprocess.run(cmd, check=True)
+        subprocess.run([nvcc, *FLAGS, "-o", out, src], check=True)
         print("built", out)
+    if harness_stale():
+        subprocess.run([nvcc, *FLAGS, "-shared", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-o", HARNESS, os.path.join(HERE, "kernel_harness.cu")],
+                       check=True)
+        print("built", HARNESS)
 
 
 if __name__ == "__main__":

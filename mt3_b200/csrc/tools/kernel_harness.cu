@@ -1,0 +1,152 @@
+// Test-only shared library (libmt3kernels.so): thin extern "C" launchers for the hot-path kernels, one kernel per call,
+// on caller-provided device pointers, on the legacy default stream.  tests/test_kernel_parity.py loads it with ctypes
+// and compares every kernel with a float64 reference at ragged shapes.  The argument structs (TcGemmArgs, GemmArgs,
+// DecGemmArgs) are passed by pointer exactly as the kernels take them, so every field is reachable from the tests;
+// kh_sizeof() lets the caller check its mirror of their layout.  Every launcher returns an MT3_* status; kh_last_error()
+// is the text behind a non-zero one.
+//
+// Built with hidden visibility: the kernel headers' inline launchers keep one-time state in function-local statics
+// (e.g. "the shared-memory attribute is set"), and exported, these would be unified with libmt3b200.so's copies when
+// both libraries are loaded into one process -- the model would then launch its own kernels without their attributes.
+// Only the kh_* entry points are exported.
+#include <stdarg.h>
+
+#include "../attention_tc.cuh"
+#include "../decode.cuh"
+#include "../gemm_simt.cuh"
+#include "../gemm_tc.cuh"
+#include "../layers.cuh"
+
+namespace mt3 {
+std::string& last_error() { static thread_local std::string e; return e; }
+int fail(int code, const char* fmt, ...) {
+  char buf[1024]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap);
+  last_error() = buf; return code;
+}
+std::atomic<uint64_t> g_launch_count{0};
+}  // namespace mt3
+
+using namespace mt3;
+
+namespace {
+
+// x -> kv_store<N> (p24 format) -> p24_elt: the exact path a K/V element takes from a GEMM epilogue into the decode
+// attention's FMAs.  code[i] = the 24 stored bits (hi16 << 8 | lo8).
+template <int N>
+__global__ void p24_roundtrip_kernel(const float* __restrict__ x, float* __restrict__ y, uint32_t* __restrict__ code, long long n) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // one group of 8 elements = one p24 chunk
+  if (g * 8 >= n) return;
+  __align__(16) char row[192];            // a whole p24 row: u16 part at 0, u8 part at 128; this group is elements 0..7
+  float v[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) v[e] = x[g * 8 + e];
+#pragma unroll
+  for (int d = 0; d < 8; d += N) kv_store<N>(row, 2, d, v + d);
+  const uint4 hi = *reinterpret_cast<const uint4*>(row);
+  const uint2 lo = *reinterpret_cast<const uint2*>(row + 128);
+  const unsigned short* h16 = reinterpret_cast<const unsigned short*>(row);
+  const unsigned char* l8 = reinterpret_cast<const unsigned char*>(row + 128);
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    y[g * 8 + e] = p24_elt(hi, lo, e);
+    code[g * 8 + e] = ((uint32_t)h16[e] << 8) | l8[e];
+  }
+}
+
+template <int FMT>
+int launch_dec_attention_fmt(const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr, int len_add,
+                             int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim,
+                             float q_eps, int pf_tiles, int B) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    attr_done = true;
+  }
+  const size_t smem = dec_attention_smem(max_len);
+  MT3_REQUIRE(smem <= 100 * 1024, MT3_ERR_UNSUPPORTED, "decode attention: max_len %d too long", max_len);
+  MT3_CUDA_CHECK(launch_kernel(dec_attention_bulk_kernel<FMT, false>, dim3(H, B), dim3(kAttThreads), smem, (cudaStream_t)0, false,
+                               q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps,
+                               (unsigned long long*)nullptr, pf_tiles));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+}  // namespace
+
+#define KH_API __attribute__((visibility("default")))
+
+extern "C" {
+
+KH_API const char* kh_last_error(void) { return last_error().c_str(); }
+
+// 0 TcGemmArgs, 1 GemmArgs, 2 DecGemmArgs
+KH_API long long kh_sizeof(int which) {
+  return which == 0 ? (long long)sizeof(TcGemmArgs) : which == 1 ? (long long)sizeof(GemmArgs) : which == 2 ? (long long)sizeof(DecGemmArgs) : -1;
+}
+
+// A [M, K] (row pitch lda), Wt = W^T [N, K] (row pitch ldw); *_lo null unless split3.  C and the epilogue from *a.
+KH_API int kh_tc_gemm(const float* a_hi, const float* a_lo, int lda, const float* w_hi, const float* w_lo, int ldw, const TcGemmArgs* a,
+               int split3) {
+  TcOperand opA, opB;
+  int r = make_operand(&opA, a_hi, a_lo, (uint64_t)a->M, (uint64_t)a->K, (uint64_t)lda);
+  if (r != MT3_OK) return r;
+  r = make_operand(&opB, w_hi, w_lo, (uint64_t)a->N, (uint64_t)a->K, (uint64_t)ldw);
+  if (r != MT3_OK) return r;
+  return launch_tc_gemm(opA, opB, *a, split3 != 0, 0);
+}
+
+KH_API int kh_sgemm(const GemmArgs* a) { return launch_sgemm(*a, 0); }
+
+// qkv [B*T, 3*H*64] (hi, lo), vt [B*H*64, T] (hi, lo; keys in vt_key_slot() order), out [B*T, H*64]
+KH_API int kh_enc_attention_tc(const float* qkv_hi, const float* qkv_lo, const float* vt_hi, const float* vt_lo, int B, int T, int H,
+                        float* out_hi, float* out_lo, int split3, float* scratch) {
+  MT3_REQUIRE(enc_attention_tc_supported(T), MT3_ERR_UNSUPPORTED, "tc attention: T=%d is not supported", T);
+  const int Q = H * 64;
+  TcOperand op, opv;
+  int r = make_operand(&op, qkv_hi, qkv_lo, (uint64_t)B * T, (uint64_t)3 * Q, (uint64_t)3 * Q);
+  if (r != MT3_OK) return r;
+  r = make_operand(&opv, vt_hi, vt_lo, (uint64_t)B * H * 64, (uint64_t)T, (uint64_t)T, 64);
+  if (r != MT3_OK) return r;
+  return launch_enc_attention_tc(op, opv, B, T, H, out_hi, out_lo, split3 != 0, 0, nullptr, scratch);
+}
+
+KH_API long long kh_enc_attention_tc_scratch_floats(int B, int T, int H) { return (long long)enc_attention_tc_scratch_floats(B, T, H); }
+KH_API int kh_enc_attention_tc_supported(int T) { return enc_attention_tc_supported(T) ? 1 : 0; }
+
+// the exact-fp32 encoder attention, launched as model.cu launches it
+KH_API int kh_enc_attention_fp32(const float* qkv, int B, int T, int H, float* out, float* out_lo) {
+  const size_t smem = (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float);
+  MT3_REQUIRE(smem <= 200 * 1024, MT3_ERR_UNSUPPORTED, "attention: T=%d too long", T);
+  MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  enc_attention_kernel<<<dim3(cdiv(T, 32), H, B), 256, smem>>>(qkv, 3 * H * 64, T, H, out, out_lo, H * 64);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+KH_API int kh_dec_gemm_cluster(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, 0, false); }
+KH_API int kh_dec_gemm(const DecGemmArgs* a) { return launch_dec_gemm(*a, 0, false); }
+KH_API int kh_dec_gemm_out_q(const DecGemmArgs* a0, const DecGemmArgs* a1) { return launch_dec_gemm_out_q(*a0, *a1, 0, false); }
+
+KH_API int kh_dec_attention(int fmt, const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr, int len_add,
+                     int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim, float q_eps,
+                     int pf_tiles, int B) {
+  switch (fmt) {
+    case 0: return launch_dec_attention_fmt<0>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
+    case 1: return launch_dec_attention_fmt<1>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
+    case 2: return launch_dec_attention_fmt<2>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
+    default: return fail(MT3_ERR_BAD_ARG, "decode attention: kv format %d", fmt);
+  }
+}
+
+// n a multiple of 8; N = 1, 2 or 4 elements per kv_store call
+KH_API int kh_p24_roundtrip(const float* x, float* y, uint32_t* code, long long n, int N) {
+  MT3_REQUIRE(n % 8 == 0 && (N == 1 || N == 2 || N == 4), MT3_ERR_BAD_ARG, "p24 roundtrip: n=%lld N=%d", n, N);
+  const unsigned grid = (unsigned)((n / 8 + 255) / 256);
+  if (N == 1) p24_roundtrip_kernel<1><<<grid, 256>>>(x, y, code, n);
+  else if (N == 2) p24_roundtrip_kernel<2><<<grid, 256>>>(x, y, code, n);
+  else p24_roundtrip_kernel<4><<<grid, 256>>>(x, y, code, n);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+}  // extern "C"
