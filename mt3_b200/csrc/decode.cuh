@@ -1,7 +1,7 @@
 // Decode-step kernels (one new token per sequence, M = batch rows), sm_90a.
 //
 // The decode step is bandwidth/latency bound (DESIGN.md "decode step"): per layer it streams 11.8 MB of fp32 weights
-// (L2-resident across steps) and, per sequence, the self-attention K/V rows written so far plus the 256 hoisted
+// (from HBM: they do not fit the 50 MB L2) and, per sequence, the self-attention K/V rows written so far plus the 256 hoisted
 // cross-attention K/V rows (HBM).  The kernels:
 //
 //  sgemm_dec_cluster_kernel   exact-fp32 GEMM for M <= 64 rows, the default.  One thread-block CLUSTER (8 CTAs; 16 for
@@ -44,6 +44,26 @@ namespace mt3 {
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void l2_prefetch_bulk(const void* gsrc, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes) : "memory");
+}
+
+// Early L2 prefetch of the next self-attention's K/V (MT3_PF_KV): the GEMM node before a layer's QKV projection pulls the
+// first rows of each of that layer's 2 B H streams (the K rows and the V rows of every (sequence, head), contiguous in the
+// head-major layout) into L2 while the HBM carries little else; the attention kernel's first bulk copies then hit L2.  Only
+// rows written by earlier steps are requested.  Only cache state changes.
+struct KvStage {
+  const char* base;                   // the layer's K/V block [B][K|V][H][cap] rows; null: off
+  const int* len_ptr; int len_add;    // rows already written: *len_ptr + len_add
+  int streams;                        // 2 B H
+  int max_rows;                       // rows per stream to prefetch
+  int row_bytes;
+  long long stream_bytes;             // cap * row_bytes
+};
+
+__device__ __forceinline__ void l2_stage_kv(const KvStage& k, unsigned cta, unsigned n_cta) {
+  if (k.base == nullptr) return;
+  const int rows = min(k.max_rows, *k.len_ptr + k.len_add);
+  if (rows <= 0) return;
+  for (int st = (int)cta; st < k.streams; st += (int)n_cta) l2_prefetch_bulk(k.base + st * k.stream_bytes, (uint32_t)(rows * k.row_bytes));
 }
 
 struct DecGemmArgs {
@@ -324,7 +344,7 @@ __device__ __forceinline__ void dec_reduce_epilogue(const DecGemmArgs& p, const 
 }
 
 template <int KC, bool TRACE, int S, int G>
-__device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x) {
+__device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x, const KvStage& kst) {
   constexpr int BM = kDecBM, BN = kDecBN, NT = 128 * G, LDA = KC + 4, LDB = kDecLDB;
   constexpr int R = BM / S;                   // rows of the tile each rank owns (8 for clusters of 8, 4 for clusters of 16)
   constexpr int KG = KC / G;                  // k-steps per warp group
@@ -378,6 +398,7 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(tc::smem_u32(&As[row * LDA + kq * 4])), "l"(src),
                  "r"(ok ? 16 : 0) : "memory");
   }
+  if (tid == 0) l2_stage_kv(kst, blockIdx.y * gridDim.x + blockIdx.x, gridDim.x * gridDim.y);
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   if (tr0) p.trace[2] = (unsigned long long)(clock64() - c0);      // loads landed
@@ -467,8 +488,8 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
 
 template <int KC, bool TRACE, int S, int G>
 __global__ void __launch_bounds__(128 * G)
-sgemm_dec_cluster_kernel(const DecGemmArgs p) {
-  dec_cluster_body<KC, TRACE, S, G>(p, (int)blockIdx.x);
+sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst) {
+  dec_cluster_body<KC, TRACE, S, G>(p, (int)blockIdx.x, kst);
 }
 
 // Two independent GEMMs that read the same inputs in ONE launch (column tiles [0, tiles0) belong to p0, the rest to
@@ -477,8 +498,8 @@ sgemm_dec_cluster_kernel(const DecGemmArgs p) {
 template <int KC0, int KC1, bool TRACE, int G>
 __global__ void __launch_bounds__(128 * G)
 sgemm_dec_cluster2_kernel(const DecGemmArgs p0, const DecGemmArgs p1, const int tiles0) {
-  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, G>(p0, (int)blockIdx.x);
-  else dec_cluster_body<KC1, TRACE, 8, G>(p1, (int)blockIdx.x - tiles0);
+  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, G>(p0, (int)blockIdx.x, KvStage{});
+  else dec_cluster_body<KC1, TRACE, 8, G>(p1, (int)blockIdx.x - tiles0, KvStage{});
 }
 
 // One warp group (128 threads) per CTA.  The body is also written for G = 2 groups that split the CTA's K chunk once
@@ -514,7 +535,7 @@ inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, c
 }
 
 template <int KC, int S, int G>
-inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, bool pdl) {
+inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst) {
   constexpr size_t smem = dec_cluster_smem<KC, G>();
   static bool attr_done = false;
   if (!attr_done) {
@@ -527,30 +548,30 @@ inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, bool
     attr_done = true;
   }
   if (a.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a, kst));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a, kst));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
 template <int G>
-inline int launch_dec_gemm_cluster_g(const DecGemmArgs& a, cudaStream_t s, bool pdl) {
+inline int launch_dec_gemm_cluster_g(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst) {
   // the long-K, narrow-N GEMM (MLP out: K = 1024, N = 512) has only N/32 x 8 = 128 CTAs at cluster size 8: a
   // cluster of 16 halves every CTA's K chunk and fills the machine
-  if ( a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, G>(a, s, pdl);
+  if ( a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, G>(a, s, pdl, kst);
   switch (a.K / 8) {
-    case 48: return launch_dec_gemm_cluster_kc<48, 8, G>(a, s, pdl);
-    case 64: return launch_dec_gemm_cluster_kc<64, 8, G>(a, s, pdl);
-    case 128: return launch_dec_gemm_cluster_kc<128, 8, G>(a, s, pdl);
+    case 48: return launch_dec_gemm_cluster_kc<48, 8, G>(a, s, pdl, kst);
+    case 64: return launch_dec_gemm_cluster_kc<64, 8, G>(a, s, pdl, kst);
+    case 128: return launch_dec_gemm_cluster_kc<128, 8, G>(a, s, pdl, kst);
     default: return MT3_ERR_UNSUPPORTED;
   }
 }
 
 // Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.
-inline int launch_dec_gemm_cluster(const DecGemmArgs& a, cudaStream_t s, bool pdl) {
+inline int launch_dec_gemm_cluster(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst = KvStage{}) {
   if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
-  return launch_dec_gemm_cluster_g<kDecGroups>(a, s, pdl);
+  return launch_dec_gemm_cluster_g<kDecGroups>(a, s, pdl, kst);
 }
 
 inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s, bool pdl = false) {
@@ -580,8 +601,10 @@ __device__ __forceinline__ float p24_elt(const uint4& hi, const uint2& lo, int e
   return __uint_as_float(__byte_perm(h, l, sel));
 }
 
-// K/V rows are read once per step and are 10x the size of L2: stream them with an evict-first policy so
-// that the 104 MB of decoder weights (re-read every step) stay L2-resident.
+// K/V rows are read once per step and are 10x the size of L2: stream them with an evict-first policy so that they do
+// not push out what is worth keeping there: the K/V tiles prefetched for this kernel's own later bulk copies (pf_tiles)
+// and for the next layer's self-attention (KvStage).  (The 104 MB of decoder weights do not fit the H100's 50 MB L2 and
+// are re-read from HBM every step.)
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));

@@ -98,6 +98,8 @@ struct Model {
   int pf_attn = 16;               // MT3_PF_ATTN=n: the decode-step attention kernels prefetch the n K/V tiles that follow their
                                   // shared-memory ring into L2 while they wait under the preceding GEMM (decode.cuh; value-neutral;
                                   // 0 = off)
+  int pf_kv = 4;        // MT3_PF_KV=n: the GEMM node before each layer's QKV projection prefetches the first n tiles of every
+                                  // K and V stream of that layer's self-attention into L2 (decode.cuh KvStage; value-neutral; 0 = off)
   int kv_fmt = 0;                 // cfg.kv_cache_format: storage format of the self and cross K/V rows (kv_dest())
   int kv_row = 256;               // bytes per K/V row of 64 elements
   // debug timeline (mt3_debug_trace_step): while `tracing` is set every decode GEMM / attention launch gets a slot
@@ -402,7 +404,7 @@ static unsigned long long* trace_slot(Model* m, const char* name) {
 // Decode-step GEMM on M = B rows: split-K exact-fp32 cluster kernel with the RMSNorm statistic fused (decode.cuh), in every
 // gemm_mode.
 static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C, int ldc,
-                    int n_split, char* kv, const int* pos, const Rows& rows, cudaStream_t s) {
+                    int n_split, char* kv, const int* pos, const Rows& rows, cudaStream_t s, const KvStage& kst = KvStage{}) {
   for (int r0 = rows.begin; r0 < rows.begin + rows.count; r0 += kDecBM) {
     DecGemmArgs a;
     memset(&a, 0, sizeof(a));
@@ -419,7 +421,7 @@ static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, in
     a.counters = m->dcounters;
     a.trace = trace_slot(m, K == m->F ? "gemm_mlp_out" : (N == 2 * m->F ? "gemm_mlp_in" : (kv ? "gemm_qkv_append" : (N == m->V ? "gemm_logits" : (K == m->Q ? "gemm_attn_out" : "gemm_cross_q")))));
     int rc = MT3_ERR_UNSUPPORTED;
-    if (m->dec_cluster) rc = launch_dec_gemm_cluster(a, s, m->pdl_gemm);
+    if (m->dec_cluster) rc = launch_dec_gemm_cluster(a, s, m->pdl_gemm, r0 == rows.begin ? kst : KvStage{});
     if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s, m->pdl_gemm);   // shapes the cluster kernel does not tile
     MT3_TRY(rc);
   }
@@ -491,6 +493,21 @@ static int dec_embed(Model* m, DecBranch& b, const int* tok_in) {
   b.y = m->dy;
   return MT3_OK;
 }
+// What the GEMM node before layer l's QKV projection prefetches of that layer's self-attention K/V; len_add: cache rows
+// written before that attention's step beyond *m->state at the time the GEMM runs (1 when the argmax kernel, which
+// advances the position, lies in between).
+static KvStage kv_stage_for(const Model* m, int l, int len_add) {
+  KvStage k{};
+  if (m->pf_kv <= 0) return k;
+  k.base = kv_layer(m, m->skv, l, m->L);
+  k.len_ptr = m->state; k.len_add = len_add;
+  k.streams = 2 * m->B * m->H;
+  k.max_rows = m->pf_kv * (m->kv_fmt == MT3_KV_F32 ? 32 : 64);
+  k.row_bytes = m->kv_row;
+  k.stream_bytes = (long long)m->L * m->kv_row;
+  return k;
+}
+
 // fused RMSNorm + QKV projection + K/V cache append (layers.py:238-240, :272-289)
 static int dec_layer_qkv(Model* m, DecBranch& b, int l) {
   return dec_gemm(m, b.y, m->D, m->dec[l].wqkv, 3 * m->Q, m->D, 1, EPI_STORE, m->dq, m->Q, m->Q, kv_layer(m, m->skv, l, m->L), m->state,
@@ -525,7 +542,8 @@ static int dec_layer_mlp(Model* m, DecBranch& b, int l) {
   const int D = m->D, Q = m->Q, F = m->F;
   MT3_TRY(dec_gemm(m, m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s));
   MT3_TRY(dec_gemm(m, b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, b.rows, b.s));
-  MT3_TRY(dec_gemm(m, m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s));
+  MT3_TRY(dec_gemm(m, m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s,
+                   l + 1 < m->Ld ? kv_stage_for(m, l + 1, 0) : KvStage{}));
   return MT3_OK;
 }
 
@@ -547,7 +565,8 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
     MT3_TRY(dec_layer_cross(m, b, l));
     MT3_TRY(dec_layer_mlp(m, b, l));
   }
-  MT3_TRY(dec_gemm(m, b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, b.rows, s));
+  MT3_TRY(dec_gemm(m, b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, b.rows, s,
+                   kv_stage_for(m, 0, 1)));
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(m->B), dim3(256), 0, s, m->pdl, (const float*)logits, m->V, m->B, m->tok_cur,
                                  m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L, (const float*)m->emb,
@@ -771,6 +790,8 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
     m->tc_attn_ok = !(e_attn && e_attn[0] == '0');
     const char* e_pfa = getenv("MT3_PF_ATTN");
     if (e_pfa) m->pf_attn = std::max(0, atoi(e_pfa));
+    const char* e_pfk = getenv("MT3_PF_KV");
+    if (e_pfk) m->pf_kv = std::max(0, atoi(e_pfk));
   }
   m->kv_fmt = cfg->kv_cache_format;
   m->kv_row = kv_row_bytes(m->kv_fmt);
