@@ -208,29 +208,35 @@ __global__ void embed_kernel(const int* __restrict__ tok, const float* __restric
 
 // ---------------------------------------------------------------------------------
 // Greedy pick + loop bookkeeping (stands in for t5x's decode loop at num_decodes=1,
-// models.py:127): next = argmax(logits) (first maximum wins, like np/jnp.argmax);
-// finished sequences emit PAD; EOS (id 1, vocabularies.py:157-159) marks finished.
+// models.py:127): next = argmax(logits), like np/jnp.argmax: the first maximum wins, and
+// the first NaN wins over every number (tracked apart from the maximum, so the common
+// all-finite path keeps its short compare chain); finished sequences emit PAD; EOS
+// (id 1, vocabularies.py:157-159) marks finished.
 // The last CTA to arrive advances the shared position and publishes all_finished.
 // state: [0] pos, [1] arrival counter, [2] all_finished
+// y_next (optional) = E[next] + PE[pos + 1], skipped at the last step, where pos + 1 = pe_rows has no PE row.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
                    int* __restrict__ finished, int* __restrict__ tokens_out, int out_ld, int* __restrict__ tok_out_user,
-                   int* __restrict__ state, int advance, int b0, const float* __restrict__ emb, const float* __restrict__ pe, int D,
-                   float* __restrict__ y_next) {
+                   int* __restrict__ state, int advance, int b0, const float* __restrict__ emb, const float* __restrict__ pe,
+                   int pe_rows, int D, float* __restrict__ y_next) {
   __shared__ float sv[8];
-  __shared__ int si[8];
+  __shared__ int si[8], snan[8];
   __shared__ int s_next[2];
   pdl_wait();
   pdl_trigger();
   // B = sequences in the whole batch (the arrival counter spans every sub-batch), b0 = first sequence of this launch
   const int b = b0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* l = logits + (long long)b * V;
+  // every number beats the start (-inf, 0x7fffffff), so bi stays out of range only when the whole row is NaN, and then
+  // nan_i = 0 replaces it
   float best = -INFINITY;
-  int bi = 0x7fffffff;
+  int bi = 0x7fffffff, nan_i = 0x7fffffff;
   for (int i = tid; i < V; i += 256) {
     const float v = l[i];
     if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+    if (v != v) nan_i = min(nan_i, i);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -238,11 +244,15 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
   }
-  if (lane == 0) { sv[warp] = best; si[warp] = bi; }
+  nan_i = __reduce_min_sync(0xffffffffu, nan_i);
+  if (lane == 0) { sv[warp] = best; si[warp] = bi; snan[warp] = nan_i; }
   __syncthreads();
   if (tid == 0) {
-    for (int w = 1; w < 8; ++w)
+    for (int w = 1; w < 8; ++w) {
       if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
+      nan_i = min(nan_i, snan[w]);
+    }
+    if (nan_i != 0x7fffffff) bi = nan_i;
     const int pos = state[0];
     int nxt = bi;
     if (finished) {
@@ -277,6 +287,7 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
   if (y_next) {
     __syncthreads();
     const int t = min(max(s_next[0], 0), V - 1), p1 = s_next[1];
+    if (p1 >= pe_rows) return;
     const float4* e = reinterpret_cast<const float4*>(emb + (long long)t * D);
     const float4* pp = reinterpret_cast<const float4*>(pe + (long long)p1 * D);
     float4* o = reinterpret_cast<float4*>(y_next + (long long)b * D);
@@ -297,15 +308,25 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
 //            live_lp / brevity_penalty(alpha, max_len)   (`finished[b]`, feeds the loop's all-finished flag).
 // tokens_out holds the LIVE sequence; beam1_finalize_kernel cuts it at the winning finish.  Ties follow the reference's
 // stable top-k (lower vocabulary id first; an existing finished hypothesis beats an equal newcomer).
+// NaN logits: candidates are ranked by cand_better, so every emitted id is in [0, V).  An all-NaN row continues with
+// id 0, the first non-EOS id of a stable top-2 over NaN scores (ids 0 and 1), and finishes nothing (the EOS candidate's
+// score is NaN).  A row that is only partly NaN makes the log-sum-exp NaN; what T5X does then depends on its NaN
+// ordering, which is not pinned here, so such rows carry no parity claim.
 // beam_f [B][2] = {live_lp, finished score}, beam_i [B] = length of the best finished hypothesis (0 = none yet).
+// y_next as in argmax_step_kernel.
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ bool cand_better(float v, int i, float ov, int oi) { return v > ov || (v == ov && i < oi); }
+// Candidate order: larger value first, NaN above every number, lower id first among equals (and among NaNs).  The
+// candidates start from (-inf, 0x7fffffff), which every real candidate beats.
+__device__ __forceinline__ bool cand_better(float v, int i, float ov, int oi) {
+  if (isnan(v)) return !isnan(ov) || i < oi;
+  return !isnan(ov) && (v > ov || (v == ov && i < oi));
+}
 
 __global__ void __launch_bounds__(256)
 beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
                   int* __restrict__ tokens_out, int out_ld, int* __restrict__ state, float* __restrict__ beam_f,
                   int* __restrict__ beam_i, float alpha, int max_len, const float* __restrict__ emb, const float* __restrict__ pe,
-                  int D, float* __restrict__ y_next) {
+                  int pe_rows, int D, float* __restrict__ y_next) {
   __shared__ float s1v[8], s2v[8], smx[8], ssum[8];
   __shared__ int s1i[8], s2i[8];
   __shared__ int s_next[2];
@@ -389,6 +410,7 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
   if (y_next) {
     __syncthreads();
     const int t = min(max(s_next[0], 0), V - 1), p1 = s_next[1];
+    if (p1 >= pe_rows) return;
     const float4* e = reinterpret_cast<const float4*>(emb + (long long)t * D);
     const float4* pp = reinterpret_cast<const float4*>(pe + (long long)p1 * D);
     float4* o = reinterpret_cast<float4*>(y_next + (long long)b * D);

@@ -113,7 +113,7 @@ struct Model {
   float* emb = nullptr;
   std::vector<DecLayer> dec;
   float* w_logits = nullptr;
-  float* pe = nullptr;            // [2048, D] sinusoid table (FixedEmbed.max_length, layers.py:565)
+  float* pe = nullptr;            // [pe_rows, D] sinusoid table (FixedEmbed.max_length, layers.py:565)
   int pe_rows = 2048;
 
   // workspace (caller-owned)
@@ -570,12 +570,12 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(m->B), dim3(256), 0, s, m->pdl, (const float*)logits, m->V, m->B, m->tok_cur,
                                  m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L, (const float*)m->emb,
-                                 (const float*)m->pe, m->D, loop_step ? m->dy : (float*)nullptr));
+                                 (const float*)m->pe, m->pe_rows, m->D, loop_step ? m->dy : (float*)nullptr));
     MT3_LAUNCH_CHECK();
   } else if (greedy) {
     MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(m->B), dim3(256), 0, s, m->pdl, (const float*)logits, m->V, m->B,
                                  use_finished ? m->tok_cur : (int*)nullptr, use_finished ? m->finished : (int*)nullptr,
-                                 tokens_ws, m->L, tok_user, m->state, 1, 0, (const float*)m->emb, (const float*)m->pe, m->D,
+                                 tokens_ws, m->L, tok_user, m->state, 1, 0, (const float*)m->emb, (const float*)m->pe, m->pe_rows, m->D,
                                  loop_step ? m->dy : (float*)nullptr));
     MT3_LAUNCH_CHECK();
   } else {
@@ -754,13 +754,13 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
   m->w_logits = take((int64_t)D * V);
   PREP(W("decoder/logits_dense/kernel"), D, V, W("decoder/decoder_norm/scale"), m->w_logits, V, 0, 1);
 #undef PREP
-  m->pe = take((int64_t)2048 * D);
+  m->pe = take((int64_t)m->pe_rows * D);
   if (rc == MT3_OK) {
     // layers.py:51-82 (float64 on the host, rounded to float32 like the reference's numpy code)
-    std::vector<float> pe((size_t)2048 * D, 0.f);
+    std::vector<float> pe((size_t)m->pe_rows * D, 0.f);
     const int half = D / 2;
     const double scale_factor = -log(10000.0 / 1.0) / (double)(half - 1);
-    for (int pos = 0; pos < 2048; ++pos)
+    for (int pos = 0; pos < m->pe_rows; ++pos)
       for (int i = 0; i < half; ++i) {
         const double div = 1.0 * exp((double)i * scale_factor);
         pe[(size_t)pos * D + i] = (float)sin((double)pos * div);

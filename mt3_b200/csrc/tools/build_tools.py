@@ -1,5 +1,5 @@
 """Builds the standalone kernel bring-up binaries and the test-only kernel harness library
-(libmt3kernels.so, loaded by tests/test_kernel_parity.py) next to this file (sm_90a).  A re-run is
+(libmt3kernels.so, loaded by tests/test_kernel_parity.py and tests/test_decode_loop_kernels.py) next to this file (sm_90a).  A re-run is
 a no-op when every output is newer than the kernel sources."""
 import os
 import subprocess

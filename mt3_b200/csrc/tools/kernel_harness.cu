@@ -1,8 +1,8 @@
 // Test-only shared library (libmt3kernels.so): thin extern "C" launchers for the hot-path kernels, one kernel per call,
-// on caller-provided device pointers, on the legacy default stream.  tests/test_kernel_parity.py loads it with ctypes
-// and compares every kernel with a float64 reference at ragged shapes.  The argument structs (TcGemmArgs, GemmArgs,
-// DecGemmArgs) are passed by pointer exactly as the kernels take them, so every field is reachable from the tests;
-// kh_sizeof() lets the caller check its mirror of their layout.  Every launcher returns an MT3_* status; kh_last_error()
+// on caller-provided device pointers, on the legacy default stream.  tests/test_kernel_parity.py and
+// tests/test_decode_loop_kernels.py load it with ctypes and compare every kernel with a float64 (or exact) reference at
+// ragged shapes.  The argument structs (TcGemmArgs, GemmArgs, DecGemmArgs) are passed by pointer exactly as the kernels
+// take them, so every field is reachable from the tests; kh_sizeof() lets the caller check its mirror of their layout.  Every launcher returns an MT3_* status; kh_last_error()
 // is the text behind a non-zero one.
 //
 // Built with hidden visibility: the kernel headers' inline launchers keep one-time state in function-local statics
@@ -145,6 +145,52 @@ KH_API int kh_p24_roundtrip(const float* x, float* y, uint32_t* code, long long 
   if (N == 1) p24_roundtrip_kernel<1><<<grid, 256>>>(x, y, code, n);
   else if (N == 2) p24_roundtrip_kernel<2><<<grid, 256>>>(x, y, code, n);
   else p24_roundtrip_kernel<4><<<grid, 256>>>(x, y, code, n);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// The decode loop's token pickers, embedding and the encoder's RMSNorm, launched with model.cu's grid and block sizes.
+// argmax_step_kernel: n_cta CTAs starting at sequence b0 (B spans the whole batch: the arrival counter advances the
+// position once all B sequences of the step have arrived, over however many launches).
+KH_API int kh_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* tok_user,
+                          int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows, int D, float* y_next,
+                          int n_cta) {
+  MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, (cudaStream_t)0, false, logits, V, B, tok_cur, finished,
+                               tokens_out, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+KH_API int kh_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
+                         float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
+                         float* y_next) {
+  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, (cudaStream_t)0, false, logits, V, B, tok_cur, finished,
+                               tokens_out, out_ld, state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i) {
+  beam1_finalize_kernel<<<B, 128>>>(tokens, B, L, steps, beam_i);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// y [b0 + n, D] rows b0 .. b0 + n - 1
+KH_API int kh_embed(const int* tok, const float* emb, int D, int V, const float* pe, const int* pos_ptr, float* y, int b0, int n) {
+  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(n), dim3(128), 0, (cudaStream_t)0, false, tok, emb, D, V, pe, pos_ptr, y, b0));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+KH_API int kh_row_rstd(const float* x, const float* x_lo, int ld, int M, int D, float eps, float* rstd) {
+  row_rstd_kernel<<<cdiv(M, 8), 256>>>(x, x_lo, ld, M, D, eps, rstd);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+KH_API int kh_rmsnorm(const float* x, const float* x_lo, int ldx, int M, int D, float eps, const float* g, float* y, int ldy) {
+  rmsnorm_kernel<<<cdiv(M, 8), 256>>>(x, x_lo, ldx, M, D, eps, g, y, ldy);
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
