@@ -81,30 +81,23 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// Same, with a thread-block cluster of (1, cluster_y, 1) CTAs.
+// Launch with a thread-block cluster of (1, cluster_y, 1) CTAs.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                                         bool pdl, unsigned cluster_y, Args... args) {
+                                         unsigned cluster_y, Args... args) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  attr[na].id = cudaLaunchAttributeClusterDimension;
-  attr[na].val.clusterDim.x = 1;
-  attr[na].val.clusterDim.y = cluster_y;
-  attr[na].val.clusterDim.z = 1;
-  ++na;
-  if (pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 1;
+  attr[0].val.clusterDim.y = cluster_y;
+  attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = na;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

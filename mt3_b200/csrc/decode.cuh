@@ -10,13 +10,12 @@
 //                      barrier, each rank sums its rows in rank order (deterministic) and runs the fused epilogue:
 //                      RMSNorm factor (statistic computed from the A tiles the GEMM loads anyway, layers.py:613-616),
 //                      residual, gated GELU, head-major KV-cache append (fp32 or fp16 cache), per-tile sums of squares
-//                      of the output.  (A second warp group per CTA splitting the K chunk once more is written in the
-//                      body as G = 2 and measured slower: kDecGroups below.)
+//                      of the output.
 //  sgemm_dec_cluster2_kernel  two such GEMMs that read the same inputs in one launch (out-projection + the
 //                      cross-attention query projection through a precomposed weight block).
-//  sgemm_dec_kernel    the same GEMM without clusters (MT3_DEC_CLUSTER=0 / shapes the cluster kernel does not
-//                      tile): K split over gridDim.y CTAs, partial tiles through an L2-resident scratch, the LAST
-//                      CTA to arrive for a tile (atomic ticket) sums them in fixed order.
+//  sgemm_dec_kernel    the same GEMM without clusters, for K the cluster kernel does not tile: K split over
+//                      gridDim.y CTAs, partial tiles through an L2-resident scratch, the LAST CTA to arrive for a
+//                      tile (atomic ticket) sums them in fixed order.
 //  dec_attention_bulk_kernel  one query per (sequence, head) over contiguous head-major K/V rows
 //                      (kv[b][K|V][head][cap][64], fp32 or fp16 elements).  A producer warp streams 8 KB tiles
 //                      (32 fp32 / 64 fp16 keys) with cp.async.bulk (TMA 1-D) into a 6-stage shared-memory ring,
@@ -262,14 +261,13 @@ sgemm_dec_kernel(const DecGemmArgs p) {
 
 // ---------------------------------------------------------------------------------------------
 // Cluster variant (the default on sm_90a): the S (8 or 16) CTAs of one 64 x 32 output tile form a thread-block
-// cluster (1, S, 1) and split K.  Each CTA computes the partial tile of its K chunk -- G groups of four warps split
-// the chunk once more and are summed through shared memory in group order -- then PUSHES the 64/S rows owned by
-// rank r into rank r's shared memory (st.shared::cluster); after ONE cluster barrier every rank sums the S partials
+// cluster (1, S, 1) and split K.  Each CTA computes the partial tile of its K chunk, then PUSHES the 64/S rows owned
+// by rank r into rank r's shared memory (st.shared::cluster); after ONE cluster barrier every rank sums the S partials
 // of its own rows from LOCAL shared memory in rank order (bit-reproducible), applies the fused epilogue and stores.
 // No global scratch, no atomics, no second barrier (nobody reads remote memory after the barrier, so a CTA may exit
 // as soon as it is done).
 //
-// Arithmetic: exact fp32 FMA, k ascending inside a group (ffma2() in common.cuh).
+// Arithmetic: exact fp32 FMA, k ascending (ffma2() in common.cuh).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_map(uint32_t smem_addr, unsigned rank) {
   uint32_t r;
@@ -285,9 +283,9 @@ __device__ __forceinline__ void st_cluster_f1(uint32_t addr, float x) {
 
 constexpr int kDecLDB = kDecBN + 8;            // padded weight rows
 constexpr int kDecRedFloats = 8 * 8 * kDecBN;  // [src rank][local rows][32 cols] partials pushed to this CTA (S*R = 64 rows)
-template <int KC, int G>
+template <int KC>
 constexpr size_t dec_cluster_smem() {
-  return (size_t)(kDecBM * (KC + 4) + KC * kDecLDB + kDecRedFloats + 64 + (G > 1 ? kDecBM * kDecBN : 0)) * sizeof(float);
+  return (size_t)(kDecBM * (KC + 4) + KC * kDecLDB + kDecRedFloats + 64) * sizeof(float);
 }
 
 // Sum this rank's 64/S rows over the S source ranks (rank order, local shared memory) and apply the fused epilogue:
@@ -343,23 +341,22 @@ __device__ __forceinline__ void dec_reduce_epilogue(const DecGemmArgs& p, const 
   }
 }
 
-template <int KC, bool TRACE, int S, int G>
+// One warp group (128 threads) per CTA: the multiply loop is bound by shared-memory bandwidth (8 LDS.128 per 64 FMAs
+// with 4 x 4 register tiles), not by issue latency, so more warps would only add a step that combines their partials.
+template <int KC, bool TRACE, int S>
 __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x, const KvStage& kst) {
-  constexpr int BM = kDecBM, BN = kDecBN, NT = 128 * G, LDA = KC + 4, LDB = kDecLDB;
+  constexpr int BM = kDecBM, BN = kDecBN, NT = 128, LDA = KC + 4, LDB = kDecLDB;
   constexpr int R = BM / S;                   // rows of the tile each rank owns (8 for clusters of 8, 4 for clusters of 16)
-  constexpr int KG = KC / G;                  // k-steps per warp group
-  static_assert(KG % 4 == 0 && (KC / (2 * G)) % 4 == 0, "K chunk must split into float4 pieces per group / per ssq thread");
+  static_assert(KC % 8 == 0, "K chunk must split into float4 pieces per ssq thread");
   extern __shared__ __align__(16) float dsm[];
   float* As = dsm;                            // [BM][LDA] activations, row-major
   float* Bs = As + BM * LDA;                  // [KC][LDB] weights
   float* Red = Bs + KC * LDB;                 // [S src][R rows][BN] partial tiles of MY rows (written by all ranks)
   float* Rss = Red + kDecRedFloats;           // [S src][R rows] partial sums of squares of my rows
-  float* Part = Rss + 64;                     // [BM][BN] partial tile of warp group 1 (G == 2)
 
   unsigned rank;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
   const int tid = threadIdx.x;
-  const int grp = tid >> 7, t128 = tid & 127;
   const int n0 = tile_x * BN;
   const int kbeg = blockIdx.y * KC;
   const bool tr = TRACE && p.trace != nullptr && tid == 0;
@@ -403,59 +400,39 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
   __syncthreads();
   if (tr0) p.trace[2] = (unsigned long long)(clock64() - c0);      // loads landed
 
-  // sum of squares of this CTA's K chunk: 2 G threads per row, each a contiguous piece, fixed butterfly order
+  // sum of squares of this CTA's K chunk: 2 threads per row, each a contiguous piece, fixed butterfly order
   float ss = 0.f;
   if (p.norm) {
-    constexpr int PIECE = KC / (2 * G);
-    const float* ar = As + (tid / (2 * G)) * LDA + (tid % (2 * G)) * PIECE;
+    constexpr int PIECE = KC / 2;
+    const float* ar = As + (tid / 2) * LDA + (tid % 2) * PIECE;
 #pragma unroll
     for (int k = 0; k < PIECE; k += 4) {
       const float4 v = *reinterpret_cast<const float4*>(ar + k);
       ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss);
     }
     ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-    if (G == 2) ss += __shfl_xor_sync(0xffffffffu, ss, 2);
   }
 
-  // ---- multiply: thread tile rows ty + 16 i (i < 4), columns tx*4 .. +3 (two float2 accumulators per row); warp
-  // group g covers k in [g KG, (g+1) KG), ascending ----
-  const int tx = t128 % 8, ty = t128 / 8;
+  // ---- multiply: thread tile rows ty + 16 i (i < 4), columns tx*4 .. +3 (two float2 accumulators per row), k
+  // ascending ----
+  const int tx = threadIdx.x % 8, ty = threadIdx.x / 8;           // unsigned: shifts without a sign fix-up
   float2 acc[4][2];
 #pragma unroll
   for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = make_float2(0.f, 0.f);
-  {
-    const float* Ag = As + grp * KG;
-    const float* Bg = Bs + grp * KG * LDB;
 #pragma unroll 4
-    for (int k = 0; k < KG; k += 4) {
-      float4 a[4], b[4];
+  for (int k = 0; k < KC; k += 4) {
+    float4 a[4], b[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(&Ag[(ty + 16 * i) * LDA + k]);
+    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(&As[(ty + 16 * i) * LDA + k]);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) b[kk] = *reinterpret_cast<const float4*>(&Bg[(k + kk) * LDB + tx * 4]);
+    for (int kk = 0; kk < 4; ++kk) b[kk] = *reinterpret_cast<const float4*>(&Bs[(k + kk) * LDB + tx * 4]);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
+    for (int i = 0; i < 4; ++i) {
+      const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          ffma2(acc[i][0], av[kk], make_float2(b[kk].x, b[kk].y));
-          ffma2(acc[i][1], av[kk], make_float2(b[kk].z, b[kk].w));
-        }
-      }
-    }
-  }
-  if (G == 2) {                                                     // group 1 -> shared memory -> added by group 0
-    if (grp == 1) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        *reinterpret_cast<float4*>(&Part[(ty + 16 * i) * BN + tx * 4]) = make_float4(acc[i][0].x, acc[i][0].y, acc[i][1].x, acc[i][1].y);
-    }
-    __syncthreads();
-    if (grp == 0) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 q = *reinterpret_cast<const float4*>(&Part[(ty + 16 * i) * BN + tx * 4]);
-        acc[i][0].x += q.x; acc[i][0].y += q.y; acc[i][1].x += q.z; acc[i][1].y += q.w;
+      for (int kk = 0; kk < 4; ++kk) {
+        ffma2(acc[i][0], av[kk], make_float2(b[kk].x, b[kk].y));
+        ffma2(acc[i][1], av[kk], make_float2(b[kk].z, b[kk].w));
       }
     }
   }
@@ -464,122 +441,107 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
 
   const uint32_t red_base = tc::smem_u32(Red) + rank * (R * BN * 4);     // my slot [rank][..] in the owner's Red
   const uint32_t rss_base = tc::smem_u32(Rss) + rank * (R * 4);
-  if (grp == 0) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {                                  // row ty + 16 i -> owner rank, local row
-      const int row = ty + 16 * i;
-      st_cluster_f4(cluster_map(red_base + (uint32_t)(((row % R) * BN + tx * 4) * 4), (unsigned)(row / R)),
-                    make_float4(acc[i][0].x, acc[i][0].y, acc[i][1].x, acc[i][1].y));
-    }
+  for (int i = 0; i < 4; ++i) {                                    // row ty + 16 i -> owner rank, local row
+    const int row = ty + 16 * i;
+    st_cluster_f4(cluster_map(red_base + (uint32_t)(((row % R) * BN + tx * 4) * 4), (unsigned)(row / R)),
+                  make_float4(acc[i][0].x, acc[i][0].y, acc[i][1].x, acc[i][1].y));
   }
-  if (p.norm && (tid % (2 * G)) == 0) {
-    const int row = tid / (2 * G);
+  if (p.norm && (tid % 2) == 0) {
+    const int row = tid / 2;
     st_cluster_f1(cluster_map(rss_base + (uint32_t)((row % R) * 4), (unsigned)(row / R)), ss);
   }
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
   if (tr0) p.trace[4] = (unsigned long long)(clock64() - c0);      // partials exchanged
 
-  if (grp == 0) dec_reduce_epilogue<S>(p, Red, Rss, rank, n0);
+  dec_reduce_epilogue<S>(p, Red, Rss, rank, n0);
   if (tr) {
     if (tr0) p.trace[5] = (unsigned long long)(clock64() - c0);    // reduce + epilogue stores issued
     atomicMax(p.trace + 1, gtime_ns());
   }
 }
 
-template <int KC, bool TRACE, int S, int G>
-__global__ void __launch_bounds__(128 * G)
+template <int KC, bool TRACE, int S>
+__global__ void __launch_bounds__(128)
 sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst) {
-  dec_cluster_body<KC, TRACE, S, G>(p, (int)blockIdx.x, kst);
+  dec_cluster_body<KC, TRACE, S>(p, (int)blockIdx.x, kst);
 }
 
 // Two independent GEMMs that read the same inputs in ONE launch (column tiles [0, tiles0) belong to p0, the rest to
 // p1): used for  y' = y + o.Wo  together with  q_raw = [o | y].[Wo.Wq ; Wq]  (the out-projection folded into the
 // next projection with a precomposed weight block), which removes a kernel from the dependency chain.
-template <int KC0, int KC1, bool TRACE, int G>
-__global__ void __launch_bounds__(128 * G)
+template <int KC0, int KC1, bool TRACE>
+__global__ void __launch_bounds__(128)
 sgemm_dec_cluster2_kernel(const DecGemmArgs p0, const DecGemmArgs p1, const int tiles0) {
-  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, G>(p0, (int)blockIdx.x, KvStage{});
-  else dec_cluster_body<KC1, TRACE, 8, G>(p1, (int)blockIdx.x - tiles0, KvStage{});
+  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8>(p0, (int)blockIdx.x, KvStage{});
+  else dec_cluster_body<KC1, TRACE, 8>(p1, (int)blockIdx.x - tiles0, KvStage{});
 }
 
-// One warp group (128 threads) per CTA.  The body is also written for G = 2 groups that split the CTA's K chunk once
-// more and are summed through shared memory: the multiply loop is bound by shared-memory bandwidth (8 LDS.128 per
-// 64 FMAs with 4 x 4 register tiles), not by issue latency, so more warps only add the combine step.
-constexpr int kDecGroups = 1;
-
-template <int KC0, int KC1, int G>
-inline int launch_dec_gemm_cluster2_g(const DecGemmArgs& a0, const DecGemmArgs& a1, cudaStream_t s, bool pdl) {
-  constexpr size_t smem = dec_cluster_smem<(KC0 > KC1 ? KC0 : KC1), G>();
+// the mt3 shapes: K = 384 (out-projection) and K = 384 + 512 (precomposed query block); MT3_ERR_UNSUPPORTED (without
+// launching) for any other
+inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, cudaStream_t s) {
+  constexpr int KC0 = 48, KC1 = 112;
+  if (a0.M > kDecBM || a1.M > kDecBM || a0.K != 8 * KC0 || a1.K != 8 * KC1 || a0.N % kDecBN != 0 || a1.N % kDecBN != 0)
+    return MT3_ERR_UNSUPPORTED;
+  constexpr size_t smem = dec_cluster_smem<KC1>();
   static bool attr_done = false;
   if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
   const int tiles0 = a0.N / kDecBN, tiles1 = a1.N / kDecBN;
   if (a0.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true, G>, dim3(tiles0 + tiles1, 8), dim3(128 * G), smem, s,
-                                         pdl, 8u, a0, a1, tiles0));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+                                         a0, a1, tiles0));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false, G>, dim3(tiles0 + tiles1, 8), dim3(128 * G), smem, s,
-                                         pdl, 8u, a0, a1, tiles0));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+                                         a0, a1, tiles0));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
-// the mt3 shapes: K = 384 (out-projection) and K = 384 + 512 (precomposed query block)
-inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, cudaStream_t s, bool pdl) {
-  if (a0.M > kDecBM || a1.M > kDecBM || a0.K != 8 * 48 || a1.K != 8 * 112 || a0.N % kDecBN != 0 || a1.N % kDecBN != 0)
-    return MT3_ERR_UNSUPPORTED;
-  return launch_dec_gemm_cluster2_g<48, 112, kDecGroups>(a0, a1, s, pdl);
-}
-
-template <int KC, int S, int G>
-inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst) {
-  constexpr size_t smem = dec_cluster_smem<KC, G>();
+template <int KC, int S>
+inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst) {
+  constexpr size_t smem = dec_cluster_smem<KC>();
   static bool attr_done = false;
   if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (S > 8) {
-      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, G>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, G>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     }
     attr_done = true;
   }
   if (a.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, G>, dim3(cdiv(a.N, kDecBN), S), dim3(128 * G), smem, s, pdl, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
-template <int G>
-inline int launch_dec_gemm_cluster_g(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst) {
+// Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.
+inline int launch_dec_gemm_cluster(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst = KvStage{}) {
+  if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
   // the long-K, narrow-N GEMM (MLP out: K = 1024, N = 512) has only N/32 x 8 = 128 CTAs at cluster size 8: a
   // cluster of 16 halves every CTA's K chunk and fills the machine
-  if ( a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, G>(a, s, pdl, kst);
+  if (a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16>(a, s, kst);
   switch (a.K / 8) {
-    case 48: return launch_dec_gemm_cluster_kc<48, 8, G>(a, s, pdl, kst);
-    case 64: return launch_dec_gemm_cluster_kc<64, 8, G>(a, s, pdl, kst);
-    case 128: return launch_dec_gemm_cluster_kc<128, 8, G>(a, s, pdl, kst);
+    case 48: return launch_dec_gemm_cluster_kc<48, 8>(a, s, kst);
+    case 64: return launch_dec_gemm_cluster_kc<64, 8>(a, s, kst);
+    case 128: return launch_dec_gemm_cluster_kc<128, 8>(a, s, kst);
     default: return MT3_ERR_UNSUPPORTED;
   }
 }
 
-// Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.
-inline int launch_dec_gemm_cluster(const DecGemmArgs& a, cudaStream_t s, bool pdl, const KvStage& kst = KvStage{}) {
-  if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
-  return launch_dec_gemm_cluster_g<kDecGroups>(a, s, pdl, kst);
-}
-
-inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s, bool pdl = false) {
+inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s) {
   MT3_REQUIRE(a.M <= kDecBM, MT3_ERR_UNSUPPORTED, "decode gemm: M=%d > %d rows", a.M, kDecBM);
   MT3_REQUIRE(a.K % kDecKC == 0 && a.K / kDecKC <= 16 && a.N % 4 == 0 && a.lda % 4 == 0 && a.ldw % 4 == 0 && a.n_split % 4 == 0,
               MT3_ERR_UNSUPPORTED, "decode gemm: K=%d must be a multiple of %d (at most 16 chunks); N=%d", a.K, kDecKC, a.N);
   MT3_REQUIRE(a.A2 == nullptr, MT3_ERR_UNSUPPORTED, "decode gemm: the two-source form needs the cluster kernel");
-  MT3_CUDA_CHECK(launch_kernel(sgemm_dec_kernel, dim3(cdiv(a.N, kDecBN), a.K / kDecKC), dim3(128), 0, s, pdl, a));
+  MT3_CUDA_CHECK(launch_kernel(sgemm_dec_kernel, dim3(cdiv(a.N, kDecBN), a.K / kDecKC), dim3(128), 0, s, false, a));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }

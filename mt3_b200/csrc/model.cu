@@ -85,16 +85,12 @@ struct Model {
   int D, H, Q, F, V, Le, Ld, L;
   float* slab = nullptr;          // all prepared weights
   float* slab_tc = nullptr;       // K-major (and hi/lo) copies for the wgmma path
-  bool fuse_q = true;             // MT3_DEC_FUSE=0: keep the self-attention out-projection and the cross-attention query
-                                  // projection as two launches (default: one launch with a precomposed weight block)
   float *dy2 = nullptr, *dssq = nullptr;   // second residual-stream buffer (ping-pong) and [B][D/32] sum-of-squares partials
   bool tc = false, split3 = false;
   TcW t_w_in;
   Act a_x, a_h, a_ao, a_g, a_enc, a_qkv, a_vt; // wgmma-path activation buffers (workspace); a_vt = per-head V^T
-  bool pdl = false;               // MT3_PDL=1: programmatic dependent launch between all decode-step kernels
-  bool pdl_attn = true;           // MT3_PDL=2 (default): only the attention launches (K/V prefetch under the preceding GEMM)
-  bool pdl_gemm = false;          // MT3_PDL=4: only the GEMM launches; bits combine (6 = attention + GEMM); 0 = off
-  bool dec_cluster = true;        // MT3_DEC_CLUSTER=0: split-K reduction through global scratch instead of DSMEM
+  bool pdl_attn = true;           // programmatic dependent launch of the decode attention kernels (K/V streamed under the
+                                  // preceding GEMM); MT3_PDL=0 turns it off, the reference for the value-neutrality tests
   int pf_attn = 16;               // MT3_PF_ATTN=n: the decode-step attention kernels prefetch the n K/V tiles that follow their
                                   // shared-memory ring into L2 while they wait under the preceding GEMM (decode.cuh; value-neutral;
                                   // 0 = off)
@@ -189,11 +185,6 @@ static int prep_copy(cudaStream_t s, const float* src, int K, int N, const float
     int _r = (expr);             \
     if (_r != MT3_OK) return _r; \
   } while (0)
-
-static int gemm(Model* m, const GemmArgs& a, cudaStream_t s) {
-  (void)m;
-  return launch_sgemm(a, s);
-}
 
 static GemmArgs gemm_args(const float* A, int lda, const float* B, int ldb, int M, int N, int K, float* C, int ldc) {
   GemmArgs a;
@@ -332,7 +323,7 @@ static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s)
   {
     GemmArgs a = gemm_args(x, m->cfg.input_depth, m->w_in, D, M, D, m->cfg.input_depth, m->h, D);
     a.epi = EPI_ADD_PE; a.pe = m->pe; a.pe_T = m->T; a.pe_ld = D;
-    MT3_TRY(gemm(m, a, s));
+    MT3_TRY(launch_sgemm(a, s));
   }
   const size_t attn_smem = (size_t)(32 * kHD + 32 * (m->T + 4) + 64 * 68) * sizeof(float);
   MT3_REQUIRE(attn_smem <= 200 * 1024, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel", m->T);
@@ -342,7 +333,7 @@ static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s)
     {
       GemmArgs a = gemm_args(m->h, D, w.wqkv, 3 * Q, M, 3 * Q, D, m->qkv, 3 * Q);
       a.row_scale = m->rstd;
-      MT3_TRY(gemm(m, a, s));
+      MT3_TRY(launch_sgemm(a, s));
     }
     {
       dim3 grid(cdiv(m->T, 32), m->H, m->B);
@@ -352,18 +343,18 @@ static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s)
     {
       GemmArgs a = gemm_args(m->ao, Q, w.wo, D, M, D, Q, m->h, D);
       a.epi = EPI_RESIDUAL; a.R = m->h; a.ldr = D;
-      MT3_TRY(gemm(m, a, s));
+      MT3_TRY(launch_sgemm(a, s));
     }
     MT3_TRY(launch_rstd(m->h, D, M, D, m->rstd, s));
     {
       GemmArgs a = gemm_args(m->h, D, w.wi, 2 * F, M, 2 * F, D, m->g, F);
       a.row_scale = m->rstd; a.epi = EPI_GATED_GELU;
-      MT3_TRY(gemm(m, a, s));
+      MT3_TRY(launch_sgemm(a, s));
     }
     {
       GemmArgs a = gemm_args(m->g, F, w.wo2, D, M, D, F, m->h, D);
       a.epi = EPI_RESIDUAL; a.R = m->h; a.ldr = D;
-      MT3_TRY(gemm(m, a, s));
+      MT3_TRY(launch_sgemm(a, s));
     }
   }
   rmsnorm_kernel<<<cdiv(M, 8), 256, 0, s>>>(m->h, nullptr, D, M, D, 1e-6f, m->enc_norm_g, encoded, D);
@@ -379,7 +370,7 @@ static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
     for (int l = 0; l < m->Ld; ++l) {
       GemmArgs a = gemm_args(encoded, D, m->dec[l].wkv_c, 2 * Q, M, 2 * Q, D, nullptr, 2 * Q);
       a.n_split = 0; a.C1 = kv_layer(m, m->ckv, l, m->T); a.kv_fmt = m->kv_fmt; a.hm_rows_per_b = m->T; a.hm_cap = m->T; a.hm_H = m->H;
-      MT3_TRY(gemm(m, a, s));
+      MT3_TRY(launch_sgemm(a, s));
     }
   }
   MT3_CUDA_CHECK(cudaMemsetAsync(m->state, 0, 4 * sizeof(int), s));
@@ -391,9 +382,6 @@ static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
   return MT3_OK;
 }
 
-// A contiguous block of sequences decoded in one launch (batches above 64 rows run in 64-row blocks).
-struct Rows { int begin, count; };
-
 constexpr int kTraceSlots = 256, kTraceWords = 16;   // words 8..15: %smid of the 8 CTAs of tile 0's cluster
 static unsigned long long* trace_slot(Model* m, const char* name) {
   if (!m->tracing || (int)m->trace_names.size() >= kTraceSlots) return nullptr;
@@ -401,14 +389,14 @@ static unsigned long long* trace_slot(Model* m, const char* name) {
   return m->trace + (size_t)(m->trace_names.size() - 1) * kTraceWords;
 }
 
-// Decode-step GEMM on M = B rows: split-K exact-fp32 cluster kernel with the RMSNorm statistic fused (decode.cuh), in every
-// gemm_mode.
+// Decode-step GEMM on M = B rows in blocks of 64: split-K exact-fp32 cluster kernel with the RMSNorm statistic fused
+// (decode.cuh), in every gemm_mode; the non-cluster kernel for K the cluster kernel does not tile.
 static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C, int ldc,
-                    int n_split, char* kv, const int* pos, const Rows& rows, cudaStream_t s, const KvStage& kst = KvStage{}) {
-  for (int r0 = rows.begin; r0 < rows.begin + rows.count; r0 += kDecBM) {
+                    int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{}) {
+  for (int r0 = 0; r0 < m->B; r0 += kDecBM) {
     DecGemmArgs a;
     memset(&a, 0, sizeof(a));
-    a.A = A + (int64_t)r0 * lda; a.lda = lda; a.W = W; a.ldw = N; a.M = std::min(kDecBM, rows.begin + rows.count - r0);
+    a.A = A + (int64_t)r0 * lda; a.lda = lda; a.W = W; a.ldw = N; a.M = std::min(kDecBM, m->B - r0);
     a.N = N; a.K = K;
     a.norm = norm; a.eps = 1e-6f; a.epi = epi;
     a.R = C + (int64_t)r0 * ldc; a.ldr = ldc;                  // residual is always added in place
@@ -420,9 +408,8 @@ static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, in
     a.partial = m->dpartial;
     a.counters = m->dcounters;
     a.trace = trace_slot(m, K == m->F ? "gemm_mlp_out" : (N == 2 * m->F ? "gemm_mlp_in" : (kv ? "gemm_qkv_append" : (N == m->V ? "gemm_logits" : (K == m->Q ? "gemm_attn_out" : "gemm_cross_q")))));
-    int rc = MT3_ERR_UNSUPPORTED;
-    if (m->dec_cluster) rc = launch_dec_gemm_cluster(a, s, m->pdl_gemm, r0 == rows.begin ? kst : KvStage{});
-    if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s, m->pdl_gemm);   // shapes the cluster kernel does not tile
+    int rc = launch_dec_gemm_cluster(a, s, r0 == 0 ? kst : KvStage{});
+    if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s);
     MT3_TRY(rc);
   }
   return MT3_OK;
@@ -431,8 +418,7 @@ static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, in
 // prefetch: the launch is part of a decode step (the kernel starts under the preceding GEMM): L2 prefetch of m->pf_attn tiles
 template <int FMT>
 static int launch_dec_attention_t(Model* m, const float* q, const char* kv, int cap, const int* len_ptr, int len_add,
-                                  float* out, const Rows& rows, cudaStream_t s, const float* q_ssq, size_t smem, int max_len,
-                                  bool prefetch) {
+                                  float* out, cudaStream_t s, const float* q_ssq, size_t smem, int max_len, bool prefetch) {
   static bool attr_done = false;
   if (!attr_done) {
     MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -440,57 +426,56 @@ static int launch_dec_attention_t(Model* m, const float* q, const char* kv, int 
     attr_done = true;
   }
   MT3_CUDA_CHECK(launch_kernel(m->tracing ? dec_attention_bulk_kernel<FMT, true> : dec_attention_bulk_kernel<FMT, false>,
-                               dim3(m->H, rows.count), dim3(kAttThreads), smem, s, m->pdl_attn,
-                               q + (int64_t)rows.begin * m->Q, m->Q, 0,
-                               (const void*)(kv + (int64_t)rows.begin * 2 * m->H * cap * m->kv_row), m->H, cap,
-                               len_ptr, len_add, max_len, out + (int64_t)rows.begin * m->Q, m->Q,
-                               q_ssq ? q_ssq + (int64_t)rows.begin * (m->D / 32) : (const float*)nullptr, m->D / 32, m->D / 32,
+                               dim3(m->H, m->B), dim3(kAttThreads), smem, s, m->pdl_attn, q, m->Q, 0, (const void*)kv, m->H, cap,
+                               len_ptr, len_add, max_len, out, m->Q, q_ssq, m->D / 32, m->D / 32,
                                (float)m->D, 1e-6f, trace_slot(m, len_ptr ? "attn_self" : "attn_cross"), prefetch ? m->pf_attn : 0));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
 static int launch_dec_attention(Model* m, const float* q, const char* kv, int cap, const int* len_ptr, int len_add,
-                                float* out, const Rows& rows, cudaStream_t s, const float* q_ssq = nullptr, bool prefetch = false) {
+                                float* out, cudaStream_t s, const float* q_ssq = nullptr, bool prefetch = false) {
   const int max_len = std::max(m->L, m->T);
   const size_t smem = dec_attention_smem(max_len);
   MT3_REQUIRE(smem <= 100 * 1024, MT3_ERR_UNSUPPORTED, "decode attention: length %d too long", max_len);
   switch (m->kv_fmt) {
-    case MT3_KV_F16: return launch_dec_attention_t<1>(m, q, kv, cap, len_ptr, len_add, out, rows, s, q_ssq, smem, max_len, prefetch);
-    case MT3_KV_P24: return launch_dec_attention_t<2>(m, q, kv, cap, len_ptr, len_add, out, rows, s, q_ssq, smem, max_len, prefetch);
-    default: return launch_dec_attention_t<0>(m, q, kv, cap, len_ptr, len_add, out, rows, s, q_ssq, smem, max_len, prefetch);
+    case MT3_KV_F16: return launch_dec_attention_t<1>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
+    case MT3_KV_P24: return launch_dec_attention_t<2>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
+    default: return launch_dec_attention_t<0>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
   }
 }
 
 // y_out = y_in + o.Wo  and  q_raw = [o | y_in].[Wo.Wq ; Wq]  in ONE launch; the RMSNorm factor of y_out is applied to
 // q inside the cross-attention kernel from the per-tile sums of squares this launch leaves in m->dssq.
-static int dec_gemm_out_q(Model* m, const DecLayer& w, const float* y_in, float* y_out, const Rows& rows, cudaStream_t s) {
+// MT3_ERR_UNSUPPORTED (nothing launched) unless B <= 64 and the mt3 widths Q = 384, D = 512.
+static int dec_gemm_out_q(Model* m, const DecLayer& w, const float* y_in, float* y_out, cudaStream_t s) {
   const int D = m->D, Q = m->Q;
-  if (rows.count > kDecBM || Q != 384 || D != 512) return MT3_ERR_UNSUPPORTED;
-  const int64_t r0 = rows.begin;
+  if (m->B > kDecBM || Q != 384 || D != 512) return MT3_ERR_UNSUPPORTED;
   DecGemmArgs a0, a1;
   memset(&a0, 0, sizeof(a0));
-  a0.A = m->dao + r0 * Q; a0.lda = Q; a0.W = w.wo; a0.ldw = D; a0.M = rows.count; a0.N = D; a0.K = Q;
-  a0.eps = 1e-6f; a0.epi = EPI_RESIDUAL; a0.R = y_in + r0 * D; a0.ldr = D; a0.C = y_out + r0 * D; a0.ldc = D; a0.n_split = D;
-  a0.ssq_out = m->dssq + r0 * (D / 32); a0.ssq_ld = D / 32;
+  a0.A = m->dao; a0.lda = Q; a0.W = w.wo; a0.ldw = D; a0.M = m->B; a0.N = D; a0.K = Q;
+  a0.eps = 1e-6f; a0.epi = EPI_RESIDUAL; a0.R = y_in; a0.ldr = D; a0.C = y_out; a0.ldc = D; a0.n_split = D;
+  a0.ssq_out = m->dssq; a0.ssq_ld = D / 32;
   a0.trace = trace_slot(m, "gemm_out+cross_q");
   memset(&a1, 0, sizeof(a1));
-  a1.A = m->dao + r0 * Q; a1.lda = Q; a1.A2 = y_in + r0 * D; a1.lda2 = D; a1.K0 = Q;
-  a1.W = w.wc1; a1.ldw = Q; a1.M = rows.count; a1.N = Q; a1.K = Q + D;
-  a1.eps = 1e-6f; a1.epi = EPI_STORE; a1.C = m->dq + r0 * Q; a1.ldc = Q; a1.n_split = Q;
+  a1.A = m->dao; a1.lda = Q; a1.A2 = y_in; a1.lda2 = D; a1.K0 = Q;
+  a1.W = w.wc1; a1.ldw = Q; a1.M = m->B; a1.N = Q; a1.K = Q + D;
+  a1.eps = 1e-6f; a1.epi = EPI_STORE; a1.C = m->dq; a1.ldc = Q; a1.n_split = Q;
   a1.R = a1.C; a1.ldr = Q;
   a1.trace = a0.trace;
-  return launch_dec_gemm_out_q(a0, a1, s, m->pdl_gemm);
+  return launch_dec_gemm_out_q(a0, a1, s);
 }
 
-// The residual stream of one step (ping-pongs between m->dy and m->dy2 across fused launches).
-struct DecBranch { Rows rows; cudaStream_t s; float* y; int fused; };
+// The state one decode step carries from layer to layer: the current residual-stream buffer (ping-pongs between m->dy
+// and m->dy2 across fused out+query launches), and whether the cross-attention query in m->dq is the fused launch's
+// un-normalised q_raw.
+struct DecBranch { float* y; bool q_raw; };
 
-static int dec_embed(Model* m, DecBranch& b, const int* tok_in) {
-  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(b.rows.count), dim3(128), 0, b.s, m->pdl, tok_in, (const float*)m->emb, m->D, m->V,
-                               (const float*)m->pe, (const int*)m->state, m->dy, b.rows.begin));
+// decoder input of the first step: E[tok_in] + PE[pos] into m->dy
+static int dec_embed(Model* m, const int* tok_in, cudaStream_t s) {
+  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(m->B), dim3(128), 0, s, false, tok_in, (const float*)m->emb, m->D, m->V,
+                               (const float*)m->pe, (const int*)m->state, m->dy, 0));
   MT3_LAUNCH_CHECK();
-  b.y = m->dy;
   return MT3_OK;
 }
 // What the GEMM node before layer l's QKV projection prefetches of that layer's self-attention K/V; len_add: cache rows
@@ -509,40 +494,39 @@ static KvStage kv_stage_for(const Model* m, int l, int len_add) {
 }
 
 // fused RMSNorm + QKV projection + K/V cache append (layers.py:238-240, :272-289)
-static int dec_layer_qkv(Model* m, DecBranch& b, int l) {
+static int dec_layer_qkv(Model* m, const DecBranch& b, int l, cudaStream_t s) {
   return dec_gemm(m, b.y, m->D, m->dec[l].wqkv, 3 * m->Q, m->D, 1, EPI_STORE, m->dq, m->Q, m->Q, kv_layer(m, m->skv, l, m->L), m->state,
-                  b.rows, b.s);
+                  s);
 }
-static int dec_layer_self(Model* m, DecBranch& b, int l) {
-  return launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, m->L), m->L, m->state, 1, m->dao, b.rows, b.s, nullptr, true);
+static int dec_layer_self(Model* m, int l, cudaStream_t s) {
+  return launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, m->L), m->L, m->state, 1, m->dao, s, nullptr, true);
 }
-// self-attention out-projection + residual, cross-attention query projection (one launch when fused)
-static int dec_layer_outq(Model* m, DecBranch& b, int l) {
+// self-attention out-projection + residual, cross-attention query projection (one launch where the fused kernel
+// takes the shape)
+static int dec_layer_outq(Model* m, DecBranch& b, int l, cudaStream_t s) {
   const DecLayer& w = m->dec[l];
   const int D = m->D, Q = m->Q;
-  b.fused = MT3_ERR_UNSUPPORTED;
-  if (m->fuse_q && m->dec_cluster) {
-    float* y_next = (b.y == m->dy) ? m->dy2 : m->dy;    // the fused launch reads y while other CTAs write y': ping-pong
-    b.fused = dec_gemm_out_q(m, w, b.y, y_next, b.rows, b.s);
-    if (b.fused == MT3_OK) b.y = y_next;
-    else if (b.fused != MT3_ERR_UNSUPPORTED) return b.fused;
+  float* y_next = (b.y == m->dy) ? m->dy2 : m->dy;      // the fused launch reads y while other CTAs write y': ping-pong
+  const int rc = dec_gemm_out_q(m, w, b.y, y_next, s);
+  b.q_raw = rc == MT3_OK;
+  if (rc == MT3_OK) {
+    b.y = y_next;
+    return MT3_OK;
   }
-  if (b.fused != MT3_OK) {
-    MT3_TRY(dec_gemm(m, m->dao, Q, w.wo, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s));
-    MT3_TRY(dec_gemm(m, b.y, D, w.wq_c, Q, D, 1, EPI_STORE, m->dq, Q, Q, nullptr, nullptr, b.rows, b.s));
-  }
-  return MT3_OK;
+  if (rc != MT3_ERR_UNSUPPORTED) return rc;
+  MT3_TRY(dec_gemm(m, m->dao, Q, w.wo, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
+  return dec_gemm(m, b.y, D, w.wq_c, Q, D, 1, EPI_STORE, m->dq, Q, Q, nullptr, nullptr, s);
 }
-static int dec_layer_cross(Model* m, DecBranch& b, int l) {
-  return launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, m->T), m->T, nullptr, m->T, m->dao, b.rows, b.s,
-                              b.fused == MT3_OK ? m->dssq : nullptr, true);
+static int dec_layer_cross(Model* m, const DecBranch& b, int l, cudaStream_t s) {
+  return launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, m->T), m->T, nullptr, m->T, m->dao, s, b.q_raw ? m->dssq : nullptr,
+                              true);
 }
-static int dec_layer_mlp(Model* m, DecBranch& b, int l) {
+static int dec_layer_mlp(Model* m, const DecBranch& b, int l, cudaStream_t s) {
   const DecLayer& w = m->dec[l];
   const int D = m->D, Q = m->Q, F = m->F;
-  MT3_TRY(dec_gemm(m, m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s));
-  MT3_TRY(dec_gemm(m, b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, b.rows, b.s));
-  MT3_TRY(dec_gemm(m, m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, b.rows, b.s,
+  MT3_TRY(dec_gemm(m, m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
+  MT3_TRY(dec_gemm(m, b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, s));
+  MT3_TRY(dec_gemm(m, m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s,
                    l + 1 < m->Ld ? kv_stage_for(m, l + 1, 0) : KvStage{}));
   return MT3_OK;
 }
@@ -555,31 +539,29 @@ static int dec_layer_mlp(Model* m, DecBranch& b, int l) {
 // step, by the previous step's argmax kernel afterwards), and this step's argmax kernel writes the next one.
 static int decode_step_impl(Model* m, const int* tok_in, float* logits, int greedy, int* tok_user, int use_finished,
                             int* tokens_ws, cudaStream_t s, bool loop_step = false) {
-  DecBranch b{Rows{0, m->B}, s, nullptr, MT3_ERR_UNSUPPORTED};
-  if (loop_step) b.y = m->dy;
-  else MT3_TRY(dec_embed(m, b, tok_in));
+  if (!loop_step) MT3_TRY(dec_embed(m, tok_in, s));
+  DecBranch b{m->dy, false};
   for (int l = 0; l < m->Ld; ++l) {
-    MT3_TRY(dec_layer_qkv(m, b, l));
-    MT3_TRY(dec_layer_self(m, b, l));
-    MT3_TRY(dec_layer_outq(m, b, l));
-    MT3_TRY(dec_layer_cross(m, b, l));
-    MT3_TRY(dec_layer_mlp(m, b, l));
+    MT3_TRY(dec_layer_qkv(m, b, l, s));
+    MT3_TRY(dec_layer_self(m, l, s));
+    MT3_TRY(dec_layer_outq(m, b, l, s));
+    MT3_TRY(dec_layer_cross(m, b, l, s));
+    MT3_TRY(dec_layer_mlp(m, b, l, s));
   }
-  MT3_TRY(dec_gemm(m, b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, b.rows, s,
-                   kv_stage_for(m, 0, 1)));
+  MT3_TRY(dec_gemm(m, b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, s, kv_stage_for(m, 0, 1)));
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
-    MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(m->B), dim3(256), 0, s, m->pdl, (const float*)logits, m->V, m->B, m->tok_cur,
+    MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(m->B), dim3(256), 0, s, false, (const float*)logits, m->V, m->B, m->tok_cur,
                                  m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L, (const float*)m->emb,
                                  (const float*)m->pe, m->pe_rows, m->D, loop_step ? m->dy : (float*)nullptr));
     MT3_LAUNCH_CHECK();
   } else if (greedy) {
-    MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(m->B), dim3(256), 0, s, m->pdl, (const float*)logits, m->V, m->B,
+    MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(m->B), dim3(256), 0, s, false, (const float*)logits, m->V, m->B,
                                  use_finished ? m->tok_cur : (int*)nullptr, use_finished ? m->finished : (int*)nullptr,
                                  tokens_ws, m->L, tok_user, m->state, 1, 0, (const float*)m->emb, (const float*)m->pe, m->pe_rows, m->D,
                                  loop_step ? m->dy : (float*)nullptr));
     MT3_LAUNCH_CHECK();
   } else {
-    MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, m->pdl, m->state));
+    MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
     MT3_LAUNCH_CHECK();
   }
   return MT3_OK;
@@ -777,15 +759,7 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
   }
   {
     const char* e_pdl = getenv("MT3_PDL");
-    // default: attention launches only (their K/V prefetch and launch latency hide under the preceding GEMM)
-    const int pdl_bits = e_pdl ? atoi(e_pdl) : 2;
-    m->pdl = (pdl_bits & 1) != 0;
-    m->pdl_attn = (pdl_bits & 3) != 0;
-    m->pdl_gemm = (pdl_bits & 5) != 0;
-    const char* e_fuse = getenv("MT3_DEC_FUSE");
-    m->fuse_q = !(e_fuse && e_fuse[0] == '0');
-    const char* e_clu = getenv("MT3_DEC_CLUSTER");
-    m->dec_cluster = !(e_clu && e_clu[0] == '0');
+    m->pdl_attn = !(e_pdl && e_pdl[0] == '0');
     const char* e_attn = getenv("MT3_TC_ATTENTION");
     m->tc_attn_ok = !(e_attn && e_attn[0] == '0');
     const char* e_pfa = getenv("MT3_PF_ATTN");
@@ -1008,10 +982,8 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
       g1 = m->graph_exec; k1 = m->graph_kernels;
     }
   }
-  if (num_steps > 0) {     // decoder input of step 0: BOS (tok_cur was zeroed by cross_kv) at position 0; later ones come from the argmax kernel
-    DecBranch b0{Rows{0, m->B}, s, nullptr, MT3_ERR_UNSUPPORTED};
-    MT3_TRY(dec_embed(m, b0, m->tok_cur));
-  }
+  if (num_steps > 0)       // decoder input of step 0: BOS (tok_cur was zeroed by cross_kv) at position 0; later ones come from the argmax kernel
+    MT3_TRY(dec_embed(m, m->tok_cur, s));
   int ran = 0;
   for (int step = 0; step < num_steps;) {
     int n = 1;
@@ -1135,16 +1107,16 @@ extern "C" int mt3_debug_launch(mt3_model* h, int32_t kind, int32_t pos, int32_t
     const int l = it % m->Ld;
     switch (kind) {
       case MT3_K_DEC_SELF_ATTN: {
-        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, L), L, nullptr, pos + 1, m->dao, Rows{0, B}, s));
+        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, L), L, nullptr, pos + 1, m->dao, s));
         break;
       }
       case MT3_K_DEC_CROSS_ATTN: {
-        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, T), T, nullptr, T, m->dao, Rows{0, B}, s));
+        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, T), T, nullptr, T, m->dao, s));
         break;
       }
       case MT3_K_DEC_QKV_GEMM: {
         // scratch output: the encoder qkv buffer (B*T rows >= B)
-        MT3_TRY(dec_gemm(m, m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->qkv, 3 * Q, 3 * Q, nullptr, nullptr, Rows{0, B}, s));
+        MT3_TRY(dec_gemm(m, m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->qkv, 3 * Q, 3 * Q, nullptr, nullptr, s));
         break;
       }
       case MT3_K_ENC_QKV_GEMM: {
@@ -1156,7 +1128,7 @@ extern "C" int mt3_debug_launch(mt3_model* h, int32_t kind, int32_t pos, int32_t
         }
         GemmArgs a = gemm_args(m->h, D, m->enc[it % std::max(1, m->Le)].wqkv, 3 * Q, M, 3 * Q, D, m->qkv, 3 * Q);
         a.row_scale = m->rstd;
-        MT3_TRY(gemm(m, a, s));
+        MT3_TRY(launch_sgemm(a, s));
         break;
       }
       case MT3_K_ENC_ATTN: {

@@ -795,13 +795,14 @@ def test_p24_codec(kh, p24_set, N):
 LOGIT_TOL = 5e-4
 
 
-def _ragged_model_check(T, B, gm, vocab, steps=4, seed=0):
+def _ragged_model_check(T, B, gm, vocab, steps=4, seed=0, emb_dim=512, num_heads=6, mlp_dim=1024):
     from mt3_b200 import network
     from oracle import mt3_oracle as O
-    ocfg = O.T5Config(vocab_size=vocab, num_encoder_layers=1, num_decoder_layers=2)
+    ocfg = O.T5Config(vocab_size=vocab, num_encoder_layers=1, num_decoder_layers=2, emb_dim=emb_dim, num_heads=num_heads,
+                      mlp_dim=mlp_dim)
     params = O.init_params(ocfg, seed=seed, norm_scale_jitter=0.05)
-    cfg = network.T5Config(vocab_size=vocab, emb_dim=512, num_heads=6, num_encoder_layers=1, num_decoder_layers=2, head_dim=64,
-                           mlp_dim=1024, mlp_activations=('gelu', 'linear'))
+    cfg = network.T5Config(vocab_size=vocab, emb_dim=emb_dim, num_heads=num_heads, num_encoder_layers=1, num_decoder_layers=2,
+                           head_dim=64, mlp_dim=mlp_dim, mlp_activations=('gelu', 'linear'))
     m = network.Transformer(cfg, params, device=DEV, max_batch=B, max_input_length=T, max_decode_length=steps + 4, gemm_mode=gm)
     audio = np.stack([O.sine_mix(T * 128, seed=500 + seed + i) for i in range(B)])
     x = O.compute_spectrogram(audio, np.float32)[:, :T]
@@ -816,7 +817,7 @@ def _ragged_model_check(T, B, gm, vocab, steps=4, seed=0):
     lg = m.teacher_forced_logits(enc, torch.from_numpy(dec_in).to(DEV).to(torch.int32)).cpu().numpy()[pick]
     scale = np.abs(l64).max()
     e = np.abs(lg - l64).max() / scale
-    print(f"model T={T} B={B} gemm={gm} vocab={vocab}: encoder {e_enc:.2e} logits {e:.2e} (of max)")
+    print(f"model T={T} B={B} gemm={gm} vocab={vocab} D={emb_dim} H={num_heads} F={mlp_dim}: encoder {e_enc:.2e} logits {e:.2e} (of max)")
     assert e_enc <= LOGIT_TOL and e <= LOGIT_TOL
     out = m.generate(torch.from_numpy(x).to(DEV), num_steps=steps, stop_at_eos=False, use_graph=False).cpu().numpy()[pick]
     srt = np.sort(l64, axis=-1)
@@ -835,11 +836,17 @@ def test_model_ragged_input_length(T, gm):
 
 
 @pytest.mark.parametrize("B,vocab", [(65, 1516), (96, 1536)])
-@pytest.mark.parametrize("cluster,pdl", [("0", "0"), ("1", "1")])
-def test_model_batch_above_64(B, vocab, cluster, pdl, monkeypatch):
+def test_model_batch_above_64(B, vocab):
     """B > 64: the decode GEMMs run in 64-row blocks and the fused out+query GEMM declines; vocab 1516 leaves the logits
     GEMM a partial 32-column tile (and the argmax / vocabulary decode a ragged row)."""
     from mt3_b200 import _lib
-    monkeypatch.setenv("MT3_DEC_CLUSTER", cluster)
-    monkeypatch.setenv("MT3_PDL", pdl)
     _ragged_model_check(32, B, _lib.GEMM_TF32X3, vocab, seed=B)
+
+
+@pytest.mark.parametrize("B", [5, 65])
+def test_model_width_off_cluster_tiling(B):
+    """4 heads (Q = 256): the self- and cross-attention out-projections (K = 256 does not split into 8 chunks of 48, 64 or
+    128) run on the non-cluster split-K decode GEMM, the other decode GEMMs on clusters, and the fused out+query GEMM
+    declines (it is built for Q = 384, D = 512)."""
+    from mt3_b200 import _lib
+    _ragged_model_check(32, B, _lib.GEMM_TF32X3, 1536, seed=B, emb_dim=512, num_heads=4, mlp_dim=1024)
