@@ -120,14 +120,12 @@ template <bool SPLIT3, bool KSPLIT, int NCHUNK>
 __global__ void __launch_bounds__(kAtThreads, 1)
 enc_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
                         const __grid_constant__ CUtensorMap tv_hi, const __grid_constant__ CUtensorMap tv_lo, int T, int H, int B,
-                        float* __restrict__ out_hi, float* __restrict__ out_lo, int ldo, float* __restrict__ dbg_S,
-                        int TK_arg, int KS_arg, float* __restrict__ part_o, float2* __restrict__ part_ml) {
+                        float* __restrict__ out_hi, float* __restrict__ out_lo, int ldo, int TK_arg, int KS_arg, float* __restrict__ part_o, float2* __restrict__ part_ml) {
   const int KS = KSPLIT ? KS_arg : 1, TK = KSPLIT ? TK_arg : T;       // compile-time 1 / T in the common single-pass form
   // TK = keys per work item (<= 256), KS = key parts per query tile (T = KS * TK).  KS == 1: the item covers all keys and
   // writes the normalised output.  KS > 1 (T = 512, ismir2021): an item covers keys [ks TK, (ks + 1) TK) and writes its
   // UNNORMALISED O tile plus (row max, row sum) to part_o / part_ml; enc_attention_combine_kernel merges the parts
   // (softmax is associative over key blocks: O = sum_k e^(m_k - m) O_k / sum_k e^(m_k - m) l_k).
-  // dbg_S (bring-up tool only): raw S rows [B][H][T][T].
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((tc::smem_u32(smem) & 1023u) != 0) __trap();          // the swizzled tiles need 1024-byte alignment
@@ -229,14 +227,6 @@ enc_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_
       }
       tc::wgmma_wait<0>();
       tc::mbar_arrive(s_done);
-      if (dbg_S && KS == 1) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          const int q = q0 + r + ((i & 2) ? 8 : 0), col = 8 * (i >> 2) + cq + (i & 1);
-          if (q < T && col < T) dbg_S[(((long long)b * H + h) * T + q) * T + col] = s0[i];
-          if (q < T && nchunk > 1 && kAtKC + col < T) dbg_S[(((long long)b * H + h) * T + q) * T + kAtKC + col] = s1[i];
-        }
-      }
       // ---- P = exp(S - rowmax), in place ----
       float mx0 = -INFINITY, mx1 = -INFINITY;
       at_chunk_max(s0, cq, TK, mx0, mx1);
@@ -338,7 +328,7 @@ inline bool enc_attention_tc_supported(int T) { return T % 8 == 0 && (T <= 2 * k
 // (out_lo optional).  T <= 256 (T % 8 == 0), or a multiple of 256 (ismir2021: 512) with `scratch`
 // (enc_attention_tc_scratch_floats) for the key-split form.
 inline int launch_enc_attention_tc(const TcOperand& qkv, const TcOperand& vt, int B, int T, int H, float* out_hi, float* out_lo,
-                                   bool split3, cudaStream_t s, float* dbg_S = nullptr, float* scratch = nullptr) {
+                                   bool split3, cudaStream_t s, float* scratch = nullptr) {
   MT3_REQUIRE(enc_attention_tc_supported(T), MT3_ERR_UNSUPPORTED, "tc attention: T=%d (needs T <= 256 and a multiple of 8, or a multiple of 256)", T);
   MT3_REQUIRE(!split3 || qkv.has_lo, MT3_ERR_BAD_ARG, "tc attention: TF32X3 needs hi/lo qkv");
   const int KS = T <= 2 * kAtKC ? 1 : T / (2 * kAtKC);
@@ -365,8 +355,8 @@ inline int launch_enc_attention_tc(const TcOperand& qkv, const TcOperand& vt, in
   const int n_items = B * H * cdiv(T, kAtQ) * KS;
   dim3 grid(n_items < sm_count ? n_items : sm_count);       // one persistent CTA per SM (192 KB of shared memory each)
 #define MT3_AT_LAUNCH(S3, KSP, NC, LO_Q, LO_V)                                                                                  \
-  enc_attention_tc_kernel<S3, KSP, NC><<<grid, kAtThreads, kAtSmem, s>>>(qkv.hi, LO_Q, vt.hi, LO_V, T, H, B, out_hi, out_lo, H * 64, dbg_S, \
-                                                                         TK, KS, part_o, part_ml)
+  enc_attention_tc_kernel<S3, KSP, NC><<<grid, kAtThreads, kAtSmem, s>>>(qkv.hi, LO_Q, vt.hi, LO_V, T, H, B, out_hi, out_lo, H * 64, TK, \
+                                                                         KS, part_o, part_ml)
   if (split3 && KS > 1) MT3_AT_LAUNCH(true, true, 2, qkv.lo, vt.lo);
   else if (split3 && nchunk > 1) MT3_AT_LAUNCH(true, false, 2, qkv.lo, vt.lo);
   else if (split3) MT3_AT_LAUNCH(true, false, 1, qkv.lo, vt.lo);

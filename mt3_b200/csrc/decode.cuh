@@ -854,4 +854,41 @@ dec_attention_bulk_kernel(const float* __restrict__ q, int ldq, int q_off, const
   }
 }
 
+using DecAttentionKernel = decltype(&dec_attention_bulk_kernel<0, false>);
+constexpr size_t kAttMaxSmem = 100 * 1024;
+
+template <int FMT>
+inline int dec_attention_kernel_fmt(bool trace, DecAttentionKernel* k) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttMaxSmem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttMaxSmem));
+    attr_done = true;
+  }
+  *k = trace ? dec_attention_bulk_kernel<FMT, true> : dec_attention_bulk_kernel<FMT, false>;
+  return MT3_OK;
+}
+
+// One CTA per (head, sequence) of a batch of B.  fmt: the K/V row format (MT3_KV_*); a trace slot selects the tracing
+// variant; pdl: the launch may start under the preceding kernel (see the producer's pdl_wait()).
+inline int launch_dec_attention(int fmt, const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr,
+                                int len_add, int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim,
+                                float q_eps, unsigned long long* trace, int pf_tiles, int B, bool pdl, cudaStream_t s) {
+  const size_t smem = dec_attention_smem(max_len);
+  MT3_REQUIRE(smem <= kAttMaxSmem, MT3_ERR_UNSUPPORTED, "decode attention: length %d too long", max_len);
+  DecAttentionKernel k = nullptr;
+  int rc;
+  switch (fmt) {
+    case MT3_KV_F32: rc = dec_attention_kernel_fmt<0>(trace != nullptr, &k); break;
+    case MT3_KV_F16: rc = dec_attention_kernel_fmt<1>(trace != nullptr, &k); break;
+    case MT3_KV_P24: rc = dec_attention_kernel_fmt<2>(trace != nullptr, &k); break;
+    default: return fail(MT3_ERR_BAD_ARG, "decode attention: kv format %d", fmt);
+  }
+  if (rc != MT3_OK) return rc;
+  MT3_CUDA_CHECK(launch_kernel(k, dim3(H, B), dim3(kAttThreads), smem, s, pdl, q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out,
+                               ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, trace, pf_tiles));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
 }  // namespace mt3

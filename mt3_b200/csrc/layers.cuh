@@ -31,6 +31,12 @@ __global__ void row_rstd_kernel(const float* __restrict__ x, const float* __rest
   if (lane == 0) rstd[row] = 1.0f / sqrtf(s / (float)D + eps);
 }
 
+inline int launch_row_rstd(const float* x, const float* x_lo, int ld, int M, int D, float eps, float* rstd, cudaStream_t s) {
+  row_rstd_kernel<<<cdiv(M, 8), 256, 0, s>>>(x, x_lo, ld, M, D, eps, rstd);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
 // y = x * rstd * g  (materialised only where the reference's API returns the normed
 // tensor itself: `encoded`, network.py:192).
 __global__ void rmsnorm_kernel(const float* __restrict__ x, const float* __restrict__ x_lo, int ldx, int M, int D,
@@ -62,6 +68,13 @@ __global__ void rmsnorm_kernel(const float* __restrict__ x, const float* __restr
     const float4 w = __ldg(gg + i);
     q[i] = make_float4(v.x * r * w.x, v.y * r * w.y, v.z * r * w.z, v.w * r * w.w);
   }
+}
+
+inline int launch_rmsnorm(const float* x, const float* x_lo, int ldx, int M, int D, float eps, const float* g, float* y, int ldy,
+                          cudaStream_t s) {
+  rmsnorm_kernel<<<cdiv(M, 8), 256, 0, s>>>(x, x_lo, ldx, M, D, eps, g, y, ldy);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
 }
 
 // ---------------------------------------------------------------------------------
@@ -185,6 +198,23 @@ enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float*
   store(q0 + tq + 16, o1);
 }
 
+// sQ, sS and sT of enc_attention_kernel; the scores of all T keys bound T.
+constexpr size_t kEncAttMaxSmem = 200 * 1024;
+inline size_t enc_attention_smem(int T) { return (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float); }
+
+inline int launch_enc_attention(const float* qkv, int ld, int T, int H, int B, float* out, float* out_lo, int ldo, cudaStream_t s) {
+  const size_t smem = enc_attention_smem(T);
+  MT3_REQUIRE(smem <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "encoder attention: T=%d too long", T);
+  static bool attr_done = false;
+  if (!attr_done) {
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
+    attr_done = true;
+  }
+  enc_attention_kernel<<<dim3(cdiv(T, 32), H, B), 256, smem, s>>>(qkv, ld, T, H, out, out_lo, ldo);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
 // ---------------------------------------------------------------------------------
 // Decoder input: y[b,:] = E[tok[b],:] + PE[pos,:]  (Embed one-hot == row gather,
 // layers.py:516-537; FixedEmbed decode branch, layers.py:589-596).
@@ -204,6 +234,14 @@ __global__ void embed_kernel(const int* __restrict__ tok, const float* __restric
     const float4 a = __ldg(e + i), c = __ldg(p + i);
     o[i] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
   }
+}
+
+// sequences b0 .. b0 + n_cta - 1
+inline int launch_embed(const int* tok, const float* emb, int D, int vocab, const float* pe, const int* pos_ptr, float* y, int b0,
+                        int n_cta, cudaStream_t s) {
+  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(n_cta), dim3(128), 0, s, false, tok, emb, D, vocab, pe, pos_ptr, y, b0));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
 }
 
 // ---------------------------------------------------------------------------------
@@ -296,6 +334,16 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
       o[i] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
     }
   }
+}
+
+// sequences b0 .. b0 + n_cta - 1 of a batch of B
+inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld,
+                              int* tok_out_user, int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows,
+                              int D, float* y_next, int n_cta, cudaStream_t s) {
+  MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
+                               out_ld, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
 }
 
 // ---------------------------------------------------------------------------------
@@ -421,6 +469,15 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
   }
 }
 
+inline int launch_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
+                             float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
+                             float* y_next, cudaStream_t s) {
+  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out, out_ld,
+                               state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
 // the best finished hypothesis = the live prefix up to its finish + EOS, zeros after; a sequence that never finished keeps
 // its live tokens (the reference returns the live beam when nothing finished)
 __global__ void beam1_finalize_kernel(int* __restrict__ tokens, int B, int L, int steps, const int* __restrict__ beam_i) {
@@ -432,6 +489,12 @@ __global__ void beam1_finalize_kernel(int* __restrict__ tokens, int B, int L, in
   }
   if (threadIdx.x == 0) tokens[(long long)b * L + n - 1] = 1;
   for (int i = n + threadIdx.x; i < L; i += blockDim.x) tokens[(long long)b * L + i] = 0;
+}
+
+inline int launch_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i, cudaStream_t s) {
+  beam1_finalize_kernel<<<B, 128, 0, s>>>(tokens, B, L, steps, beam_i);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
 }
 
 // ---------------------------------------------------------------------------------

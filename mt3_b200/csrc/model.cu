@@ -88,7 +88,8 @@ struct Model {
   float *dy2 = nullptr, *dssq = nullptr;   // second residual-stream buffer (ping-pong) and [B][D/32] sum-of-squares partials
   bool tc = false, split3 = false;
   TcW t_w_in;
-  Act a_x, a_h, a_ao, a_g, a_enc, a_qkv, a_vt; // wgmma-path activation buffers (workspace); a_vt = per-head V^T
+  Act a_h, a_ao, a_g, a_qkv;      // encoder activations (workspace), in every mode; lo planes in TF32X3 mode only
+  Act a_x, a_enc, a_vt;           // wgmma path only: TF32X3 splits of the caller's encoder input and of `encoded`; per-head V^T
   bool pdl_attn = true;           // programmatic dependent launch of the decode attention kernels (K/V streamed under the
                                   // preceding GEMM); MT3_PDL=0 turns it off, the reference for the value-neutrality tests
   int pf_attn = 16;               // MT3_PF_ATTN=n: the decode-step attention kernels prefetch the n K/V tiles that follow their
@@ -186,28 +187,6 @@ static int prep_copy(cudaStream_t s, const float* src, int K, int N, const float
     if (_r != MT3_OK) return _r; \
   } while (0)
 
-static GemmArgs gemm_args(const float* A, int lda, const float* B, int ldb, int M, int N, int K, float* C, int ldc) {
-  GemmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.A = A; a.lda = lda; a.B = B; a.ldb = ldb; a.M = M; a.N = N; a.K = K;
-  a.C = C; a.ldc = ldc; a.n_split = N; a.epi = EPI_STORE;
-  return a;
-}
-
-static int launch_rstd(const float* x, int ld, int M, int D, float* rstd, cudaStream_t s) {
-  row_rstd_kernel<<<cdiv(M, 8), 256, 0, s>>>(x, nullptr, ld, M, D, 1e-6f, rstd);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
-}
-
-static int set_attr_once() {
-  static bool done = false;
-  if (done) return MT3_OK;
-  MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  done = true;
-  return MT3_OK;
-}
-
 static int prep_tc_weight(Model* m, cudaStream_t s, const float* w, int K, int N, float*& cursor, TcW* out) {
   out->K = K; out->N = N;
   out->hi = cursor; cursor += (int64_t)K * N;
@@ -225,153 +204,116 @@ static int64_t tc_weight_floats(const mt3_model_config& c) {
   return n * (c.gemm_mode == MT3_GEMM_TF32X3 ? 2 : 1);
 }
 
-static TcGemmArgs tc_args(int M, int N, int K, float* C_hi, float* C_lo, int ldc) {
+// The epilogue of an encoder-side GEMM C[M, N] = A[M, K] . W[K, N], in the wgmma kernel's terms (enc_gemm() maps it onto
+// the SIMT kernel's).
+static TcGemmArgs gemm_epi(int M, int N, int K, float* C_hi, float* C_lo, int ldc) {
   TcGemmArgs a;
   memset(&a, 0, sizeof(a));
   a.M = M; a.N = N; a.K = K; a.C_hi = C_hi; a.C_lo = C_lo; a.ldc = ldc; a.n_split = N; a.epi = EPI_STORE;
   return a;
 }
 
-// Encoder on the wgmma path.  Activations that feed a GEMM are kept as tf32 hi/lo pairs in TF32X3 mode.
-static int encode_tc_impl(Model* m, const float* x, float* encoded, cudaStream_t s) {
-  const int M = m->B * m->T, D = m->D, Q = m->Q, F = m->F, depth = m->cfg.input_depth;
-  MT3_TRY(set_attr_once());
-  TcOperand opx;
-  if (m->split3) {
-    const long long n4 = (long long)M * depth / 4;
-    split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(x, m->a_x.hi, m->a_x.lo, n4);
-    MT3_LAUNCH_CHECK();
-    opx = m->a_x.op;
-  } else {
-    MT3_TRY(make_operand(&opx, x, nullptr, M, depth, depth));
-  }
-  {
-    TcGemmArgs a = tc_args(M, D, depth, m->a_h.hi, m->a_h.lo, D);
-    a.epi = EPI_ADD_PE; a.pe = m->pe; a.pe_T = m->T; a.pe_ld = D;
-    MT3_TRY(launch_tc_gemm(opx, m->t_w_in.op, a, m->split3, s));
-  }
-  const size_t attn_smem = (size_t)(32 * kHD + 32 * (m->T + 4) + 64 * 68) * sizeof(float);
-  MT3_REQUIRE(attn_smem <= 200 * 1024, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel", m->T);
-  const bool tc_attn = m->tc_attn_ok && enc_attention_tc_supported(m->T);
-  for (int l = 0; l < m->Le; ++l) {
-    const EncLayer& w = m->enc[l];
-    row_rstd_kernel<<<cdiv(M, 8), 256, 0, s>>>(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->rstd);
-    MT3_LAUNCH_CHECK();
-    {
-      // qkv goes out as a tf32 hi/lo pair when the wgmma attention kernel consumes it
-      TcGemmArgs a = tc_args(M, 3 * Q, D, m->qkv, tc_attn ? m->a_qkv.lo : nullptr, 3 * Q);
-      a.row_scale = m->rstd;
-      if (tc_attn) {   // the V third goes out transposed per head: the K-major operand of P.V
-        a.VT_hi = m->a_vt.hi; a.VT_lo = m->a_vt.lo; a.vt_col0 = 2 * Q; a.vt_T = m->T; a.vt_H = m->H;
-      }
-      MT3_TRY(launch_tc_gemm(m->a_h.op, w.t_wqkv.op, a, m->split3, s));
-    }
-    if (tc_attn) {
-      MT3_TRY(launch_enc_attention_tc(m->a_qkv.op, m->a_vt.op, m->B, m->T, m->H, m->a_ao.hi, m->a_ao.lo, m->split3, s, nullptr,
-                                      m->att_scratch));
-    } else {
-      enc_attention_kernel<<<dim3(cdiv(m->T, 32), m->H, m->B), 256, attn_smem, s>>>(m->qkv, 3 * Q, m->T, m->H, m->a_ao.hi,
-                                                                                     m->a_ao.lo, Q);
-      MT3_LAUNCH_CHECK();
-    }
-    {
-      TcGemmArgs a = tc_args(M, D, Q, m->a_h.hi, m->a_h.lo, D);
-      a.epi = EPI_RESIDUAL; a.R_hi = m->a_h.hi; a.R_lo = m->a_h.lo; a.ldr = D;
-      MT3_TRY(launch_tc_gemm(m->a_ao.op, w.t_wo.op, a, m->split3, s));
-    }
-    row_rstd_kernel<<<cdiv(M, 8), 256, 0, s>>>(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->rstd);
-    MT3_LAUNCH_CHECK();
-    {
-      TcGemmArgs a = tc_args(M, 2 * F, D, m->a_g.hi, m->a_g.lo, F);
-      a.row_scale = m->rstd; a.epi = EPI_GATED_GELU;
-      MT3_TRY(launch_tc_gemm(m->a_h.op, w.t_wi.op, a, m->split3, s));
-    }
-    {
-      TcGemmArgs a = tc_args(M, D, F, m->a_h.hi, m->a_h.lo, D);
-      a.epi = EPI_RESIDUAL; a.R_hi = m->a_h.hi; a.R_lo = m->a_h.lo; a.ldr = D;
-      MT3_TRY(launch_tc_gemm(m->a_g.op, w.t_wo2.op, a, m->split3, s));
-    }
-  }
-  rmsnorm_kernel<<<cdiv(M, 8), 256, 0, s>>>(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->enc_norm_g, encoded, D);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+// One encoder-side GEMM on the back end gemm_mode picks: wgmma on the K-major copy tw, or the SIMT kernel on the row-major
+// w.  A is dense (row pitch K), w has row pitch N.  Activations that feed a GEMM are carried as tf32 hi/lo pairs in TF32X3
+// mode only, and the V^T store only feeds the wgmma attention, so the SIMT kernel never sees a lo plane or V^T.
+static int enc_gemm(const Model* m, const Act& A, const float* w, const TcW& tw, const TcGemmArgs& e, cudaStream_t s) {
+  if (m->tc) return launch_tc_gemm(A.op, tw.op, e, m->split3, s);
+  GemmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.A = A.hi; a.lda = e.K; a.B = w; a.ldb = e.N; a.M = e.M; a.N = e.N; a.K = e.K;
+  a.row_scale = e.row_scale; a.epi = e.epi; a.R = e.R_hi; a.ldr = e.ldr; a.pe = e.pe; a.pe_T = e.pe_T; a.pe_ld = e.pe_ld;
+  a.C = e.C_hi; a.ldc = e.ldc;
+  a.n_split = e.n_split; a.C1 = e.C1; a.kv_fmt = e.kv_fmt; a.hm_rows_per_b = e.hm_rows_per_b; a.hm_cap = e.hm_cap; a.hm_H = e.hm_H;
+  a.hm_pos = e.hm_pos;
+  return launch_sgemm(a, s);
 }
 
-static int cross_kv_tc_impl(Model* m, const float* encoded, cudaStream_t s) {
-  const int M = m->B * m->T, D = m->D, Q = m->Q;
-  TcOperand ope;
+// x [B*T, K], owned by the caller, as the A operand of an encoder-side GEMM; in TF32X3 mode it is split into `pair` first.
+static int enc_input(const Model* m, const float* x, int K, const Act& pair, Act* out, cudaStream_t s) {
+  const int M = m->B * m->T;
   if (m->split3) {
-    const long long n4 = (long long)M * D / 4;
-    split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(encoded, m->a_enc.hi, m->a_enc.lo, n4);
+    const long long n4 = (long long)M * K / 4;
+    split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(x, pair.hi, pair.lo, n4);
     MT3_LAUNCH_CHECK();
-    ope = m->a_enc.op;
-  } else {
-    MT3_TRY(make_operand(&ope, encoded, nullptr, M, D, D));
+    *out = pair;
+    return MT3_OK;
   }
-  for (int l = 0; l < m->Ld; ++l) {
-    TcGemmArgs a = tc_args(M, 2 * Q, D, nullptr, nullptr, 2 * Q);
-    a.n_split = 0; a.C1 = kv_layer(m, m->ckv, l, m->T); a.kv_fmt = m->kv_fmt; a.hm_rows_per_b = m->T; a.hm_cap = m->T; a.hm_H = m->H;
-    MT3_TRY(launch_tc_gemm(ope, m->dec[l].t_wkv_c.op, a, m->split3, s));
-  }
-  return MT3_OK;
+  out->hi = const_cast<float*>(x);
+  return m->tc ? make_operand(&out->op, x, nullptr, M, K, K) : MT3_OK;
 }
 
+static bool enc_tc_attention(const Model* m) { return m->tc && m->tc_attn_ok && enc_attention_tc_supported(m->T); }
+
+// Encoder layer steps (network.py:44-85).  RMSNorm statistic of the residual stream h, applied as the next GEMM's row scale
+static int enc_rstd(Model* m, cudaStream_t s) {
+  return launch_row_rstd(m->a_h.hi, m->a_h.lo, m->D, m->B * m->T, m->D, 1e-6f, m->rstd, s);
+}
+// QKV projection.  When the wgmma attention consumes qkv it goes out as a tf32 hi/lo pair (TF32X3), and the V third also
+// transposed per head: the K-major operand of P.V.
+static int enc_layer_qkv(Model* m, int l, cudaStream_t s) {
+  const int Q = m->Q;
+  const bool tc_attn = enc_tc_attention(m);
+  TcGemmArgs a = gemm_epi(m->B * m->T, 3 * Q, m->D, m->a_qkv.hi, tc_attn ? m->a_qkv.lo : nullptr, 3 * Q);
+  a.row_scale = m->rstd;
+  if (tc_attn) {
+    a.VT_hi = m->a_vt.hi; a.VT_lo = m->a_vt.lo; a.vt_col0 = 2 * Q; a.vt_T = m->T; a.vt_H = m->H;
+  }
+  return enc_gemm(m, m->a_h, m->enc[l].wqkv, m->enc[l].t_wqkv, a, s);
+}
+static int enc_layer_attn(Model* m, cudaStream_t s) {
+  if (enc_tc_attention(m))
+    return launch_enc_attention_tc(m->a_qkv.op, m->a_vt.op, m->B, m->T, m->H, m->a_ao.hi, m->a_ao.lo, m->split3, s, m->att_scratch);
+  return launch_enc_attention(m->a_qkv.hi, 3 * m->Q, m->T, m->H, m->B, m->a_ao.hi, m->a_ao.lo, m->Q, s);
+}
+// h += A . W: the attention out-projection (A = ao) and the MLP out-projection (A = g)
+static int enc_layer_residual(Model* m, const Act& A, int K, const float* w, const TcW& tw, cudaStream_t s) {
+  const int D = m->D;
+  TcGemmArgs a = gemm_epi(m->B * m->T, D, K, m->a_h.hi, m->a_h.lo, D);
+  a.epi = EPI_RESIDUAL; a.R_hi = m->a_h.hi; a.R_lo = m->a_h.lo; a.ldr = D;
+  return enc_gemm(m, A, w, tw, a, s);
+}
+static int enc_layer_mlp_in(Model* m, int l, cudaStream_t s) {
+  const int F = m->F;
+  TcGemmArgs a = gemm_epi(m->B * m->T, 2 * F, m->D, m->a_g.hi, m->a_g.lo, F);
+  a.row_scale = m->rstd; a.epi = EPI_GATED_GELU;
+  return enc_gemm(m, m->a_h, m->enc[l].wi, m->enc[l].t_wi, a, s);
+}
+
+// Encoder (network.py:158-193): input projection + PE, the layers, and the closing RMSNorm into `encoded`.
 static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s) {
-  if (m->tc) return encode_tc_impl(m, x, encoded, s);
-  const int M = m->B * m->T, D = m->D, Q = m->Q, F = m->F;
-  MT3_TRY(set_attr_once());
+  const int M = m->B * m->T, D = m->D, depth = m->cfg.input_depth;
+  // the exact-fp32 attention kernel's limit, in every mode
+  MT3_REQUIRE(enc_attention_smem(m->T) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel",
+              m->T);
+  Act ax;
+  MT3_TRY(enc_input(m, x, depth, m->a_x, &ax, s));
   {
-    GemmArgs a = gemm_args(x, m->cfg.input_depth, m->w_in, D, M, D, m->cfg.input_depth, m->h, D);
+    TcGemmArgs a = gemm_epi(M, D, depth, m->a_h.hi, m->a_h.lo, D);
     a.epi = EPI_ADD_PE; a.pe = m->pe; a.pe_T = m->T; a.pe_ld = D;
-    MT3_TRY(launch_sgemm(a, s));
+    MT3_TRY(enc_gemm(m, ax, m->w_in, m->t_w_in, a, s));
   }
-  const size_t attn_smem = (size_t)(32 * kHD + 32 * (m->T + 4) + 64 * 68) * sizeof(float);
-  MT3_REQUIRE(attn_smem <= 200 * 1024, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel", m->T);
   for (int l = 0; l < m->Le; ++l) {
     const EncLayer& w = m->enc[l];
-    MT3_TRY(launch_rstd(m->h, D, M, D, m->rstd, s));
-    {
-      GemmArgs a = gemm_args(m->h, D, w.wqkv, 3 * Q, M, 3 * Q, D, m->qkv, 3 * Q);
-      a.row_scale = m->rstd;
-      MT3_TRY(launch_sgemm(a, s));
-    }
-    {
-      dim3 grid(cdiv(m->T, 32), m->H, m->B);
-      enc_attention_kernel<<<grid, 256, attn_smem, s>>>(m->qkv, 3 * Q, m->T, m->H, m->ao, nullptr, Q);
-      MT3_LAUNCH_CHECK();
-    }
-    {
-      GemmArgs a = gemm_args(m->ao, Q, w.wo, D, M, D, Q, m->h, D);
-      a.epi = EPI_RESIDUAL; a.R = m->h; a.ldr = D;
-      MT3_TRY(launch_sgemm(a, s));
-    }
-    MT3_TRY(launch_rstd(m->h, D, M, D, m->rstd, s));
-    {
-      GemmArgs a = gemm_args(m->h, D, w.wi, 2 * F, M, 2 * F, D, m->g, F);
-      a.row_scale = m->rstd; a.epi = EPI_GATED_GELU;
-      MT3_TRY(launch_sgemm(a, s));
-    }
-    {
-      GemmArgs a = gemm_args(m->g, F, w.wo2, D, M, D, F, m->h, D);
-      a.epi = EPI_RESIDUAL; a.R = m->h; a.ldr = D;
-      MT3_TRY(launch_sgemm(a, s));
-    }
+    MT3_TRY(enc_rstd(m, s));
+    MT3_TRY(enc_layer_qkv(m, l, s));
+    MT3_TRY(enc_layer_attn(m, s));
+    MT3_TRY(enc_layer_residual(m, m->a_ao, m->Q, w.wo, w.t_wo, s));
+    MT3_TRY(enc_rstd(m, s));
+    MT3_TRY(enc_layer_mlp_in(m, l, s));
+    MT3_TRY(enc_layer_residual(m, m->a_g, m->F, w.wo2, w.t_wo2, s));
   }
-  rmsnorm_kernel<<<cdiv(M, 8), 256, 0, s>>>(m->h, nullptr, D, M, D, 1e-6f, m->enc_norm_g, encoded, D);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_rmsnorm(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->enc_norm_g, encoded, D, s);
 }
 
+// The hoisted cross-attention K/V of every decoder layer, head-major, and the reset of the decode state.
 static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
   const int M = m->B * m->T, D = m->D, Q = m->Q;
-  if (m->tc) {
-    MT3_TRY(cross_kv_tc_impl(m, encoded, s));
-  } else {
-    for (int l = 0; l < m->Ld; ++l) {
-      GemmArgs a = gemm_args(encoded, D, m->dec[l].wkv_c, 2 * Q, M, 2 * Q, D, nullptr, 2 * Q);
-      a.n_split = 0; a.C1 = kv_layer(m, m->ckv, l, m->T); a.kv_fmt = m->kv_fmt; a.hm_rows_per_b = m->T; a.hm_cap = m->T; a.hm_H = m->H;
-      MT3_TRY(launch_sgemm(a, s));
-    }
+  Act ae;
+  MT3_TRY(enc_input(m, encoded, D, m->a_enc, &ae, s));
+  for (int l = 0; l < m->Ld; ++l) {
+    TcGemmArgs a = gemm_epi(M, 2 * Q, D, nullptr, nullptr, 2 * Q);
+    a.n_split = 0; a.C1 = kv_layer(m, m->ckv, l, m->T); a.kv_fmt = m->kv_fmt; a.hm_rows_per_b = m->T; a.hm_cap = m->T; a.hm_H = m->H;
+    MT3_TRY(enc_gemm(m, ae, m->dec[l].wkv_c, m->dec[l].t_wkv_c, a, s));
   }
   MT3_CUDA_CHECK(cudaMemsetAsync(m->state, 0, 4 * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->dcounters, 0, (size_t)m->dcounters_n * sizeof(int), s));
@@ -391,8 +333,9 @@ static unsigned long long* trace_slot(Model* m, const char* name) {
 
 // Decode-step GEMM on M = B rows in blocks of 64: split-K exact-fp32 cluster kernel with the RMSNorm statistic fused
 // (decode.cuh), in every gemm_mode; the non-cluster kernel for K the cluster kernel does not tile.
-static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C, int ldc,
-                    int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{}) {
+// name: the node's trace name (mt3_debug_trace_step).
+static int dec_gemm(Model* m, const char* name, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C,
+                    int ldc, int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{}) {
   for (int r0 = 0; r0 < m->B; r0 += kDecBM) {
     DecGemmArgs a;
     memset(&a, 0, sizeof(a));
@@ -407,7 +350,7 @@ static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, in
     }
     a.partial = m->dpartial;
     a.counters = m->dcounters;
-    a.trace = trace_slot(m, K == m->F ? "gemm_mlp_out" : (N == 2 * m->F ? "gemm_mlp_in" : (kv ? "gemm_qkv_append" : (N == m->V ? "gemm_logits" : (K == m->Q ? "gemm_attn_out" : "gemm_cross_q")))));
+    a.trace = trace_slot(m, name);
     int rc = launch_dec_gemm_cluster(a, s, r0 == 0 ? kst : KvStage{});
     if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s);
     MT3_TRY(rc);
@@ -416,33 +359,11 @@ static int dec_gemm(Model* m, const float* A, int lda, const float* W, int N, in
 }
 
 // prefetch: the launch is part of a decode step (the kernel starts under the preceding GEMM): L2 prefetch of m->pf_attn tiles
-template <int FMT>
-static int launch_dec_attention_t(Model* m, const float* q, const char* kv, int cap, const int* len_ptr, int len_add,
-                                  float* out, cudaStream_t s, const float* q_ssq, size_t smem, int max_len, bool prefetch) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr_done = true;
-  }
-  MT3_CUDA_CHECK(launch_kernel(m->tracing ? dec_attention_bulk_kernel<FMT, true> : dec_attention_bulk_kernel<FMT, false>,
-                               dim3(m->H, m->B), dim3(kAttThreads), smem, s, m->pdl_attn, q, m->Q, 0, (const void*)kv, m->H, cap,
-                               len_ptr, len_add, max_len, out, m->Q, q_ssq, m->D / 32, m->D / 32,
-                               (float)m->D, 1e-6f, trace_slot(m, len_ptr ? "attn_self" : "attn_cross"), prefetch ? m->pf_attn : 0));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
-}
-
-static int launch_dec_attention(Model* m, const float* q, const char* kv, int cap, const int* len_ptr, int len_add,
-                                float* out, cudaStream_t s, const float* q_ssq = nullptr, bool prefetch = false) {
-  const int max_len = std::max(m->L, m->T);
-  const size_t smem = dec_attention_smem(max_len);
-  MT3_REQUIRE(smem <= 100 * 1024, MT3_ERR_UNSUPPORTED, "decode attention: length %d too long", max_len);
-  switch (m->kv_fmt) {
-    case MT3_KV_F16: return launch_dec_attention_t<1>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
-    case MT3_KV_P24: return launch_dec_attention_t<2>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
-    default: return launch_dec_attention_t<0>(m, q, kv, cap, len_ptr, len_add, out, s, q_ssq, smem, max_len, prefetch);
-  }
+static int dec_attention(Model* m, const float* q, const char* kv, int cap, const int* len_ptr, int len_add, float* out, cudaStream_t s,
+                         const float* q_ssq = nullptr, bool prefetch = false) {
+  return launch_dec_attention(m->kv_fmt, q, m->Q, 0, kv, m->H, cap, len_ptr, len_add, std::max(m->L, m->T), out, m->Q, q_ssq, m->D / 32,
+                              m->D / 32, (float)m->D, 1e-6f, trace_slot(m, len_ptr ? "attn_self" : "attn_cross"),
+                              prefetch ? m->pf_attn : 0, m->B, m->pdl_attn, s);
 }
 
 // y_out = y_in + o.Wo  and  q_raw = [o | y_in].[Wo.Wq ; Wq]  in ONE launch; the RMSNorm factor of y_out is applied to
@@ -473,10 +394,7 @@ struct DecBranch { float* y; bool q_raw; };
 
 // decoder input of the first step: E[tok_in] + PE[pos] into m->dy
 static int dec_embed(Model* m, const int* tok_in, cudaStream_t s) {
-  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(m->B), dim3(128), 0, s, false, tok_in, (const float*)m->emb, m->D, m->V,
-                               (const float*)m->pe, (const int*)m->state, m->dy, 0));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_embed(tok_in, m->emb, m->D, m->V, m->pe, m->state, m->dy, 0, m->B, s);
 }
 // What the GEMM node before layer l's QKV projection prefetches of that layer's self-attention K/V; len_add: cache rows
 // written before that attention's step beyond *m->state at the time the GEMM runs (1 when the argmax kernel, which
@@ -495,11 +413,11 @@ static KvStage kv_stage_for(const Model* m, int l, int len_add) {
 
 // fused RMSNorm + QKV projection + K/V cache append (layers.py:238-240, :272-289)
 static int dec_layer_qkv(Model* m, const DecBranch& b, int l, cudaStream_t s) {
-  return dec_gemm(m, b.y, m->D, m->dec[l].wqkv, 3 * m->Q, m->D, 1, EPI_STORE, m->dq, m->Q, m->Q, kv_layer(m, m->skv, l, m->L), m->state,
-                  s);
+  return dec_gemm(m, "gemm_qkv_append", b.y, m->D, m->dec[l].wqkv, 3 * m->Q, m->D, 1, EPI_STORE, m->dq, m->Q, m->Q,
+                  kv_layer(m, m->skv, l, m->L), m->state, s);
 }
 static int dec_layer_self(Model* m, int l, cudaStream_t s) {
-  return launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, m->L), m->L, m->state, 1, m->dao, s, nullptr, true);
+  return dec_attention(m, m->dq, kv_layer(m, m->skv, l, m->L), m->L, m->state, 1, m->dao, s, nullptr, true);
 }
 // self-attention out-projection + residual, cross-attention query projection (one launch where the fused kernel
 // takes the shape)
@@ -514,19 +432,18 @@ static int dec_layer_outq(Model* m, DecBranch& b, int l, cudaStream_t s) {
     return MT3_OK;
   }
   if (rc != MT3_ERR_UNSUPPORTED) return rc;
-  MT3_TRY(dec_gemm(m, m->dao, Q, w.wo, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
-  return dec_gemm(m, b.y, D, w.wq_c, Q, D, 1, EPI_STORE, m->dq, Q, Q, nullptr, nullptr, s);
+  MT3_TRY(dec_gemm(m, "gemm_attn_out", m->dao, Q, w.wo, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
+  return dec_gemm(m, "gemm_cross_q", b.y, D, w.wq_c, Q, D, 1, EPI_STORE, m->dq, Q, Q, nullptr, nullptr, s);
 }
 static int dec_layer_cross(Model* m, const DecBranch& b, int l, cudaStream_t s) {
-  return launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, m->T), m->T, nullptr, m->T, m->dao, s, b.q_raw ? m->dssq : nullptr,
-                              true);
+  return dec_attention(m, m->dq, kv_layer(m, m->ckv, l, m->T), m->T, nullptr, m->T, m->dao, s, b.q_raw ? m->dssq : nullptr, true);
 }
 static int dec_layer_mlp(Model* m, const DecBranch& b, int l, cudaStream_t s) {
   const DecLayer& w = m->dec[l];
   const int D = m->D, Q = m->Q, F = m->F;
-  MT3_TRY(dec_gemm(m, m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
-  MT3_TRY(dec_gemm(m, b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, s));
-  MT3_TRY(dec_gemm(m, m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s,
+  MT3_TRY(dec_gemm(m, "gemm_attn_out", m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
+  MT3_TRY(dec_gemm(m, "gemm_mlp_in", b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, s));
+  MT3_TRY(dec_gemm(m, "gemm_mlp_out", m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s,
                    l + 1 < m->Ld ? kv_stage_for(m, l + 1, 0) : KvStage{}));
   return MT3_OK;
 }
@@ -548,18 +465,15 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
     MT3_TRY(dec_layer_cross(m, b, l, s));
     MT3_TRY(dec_layer_mlp(m, b, l, s));
   }
-  MT3_TRY(dec_gemm(m, b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, s, kv_stage_for(m, 0, 1)));
+  MT3_TRY(dec_gemm(m, "gemm_logits", b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, s,
+                   kv_stage_for(m, 0, 1)));
+  float* y_next = loop_step ? m->dy : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
-    MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(m->B), dim3(256), 0, s, false, (const float*)logits, m->V, m->B, m->tok_cur,
-                                 m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L, (const float*)m->emb,
-                                 (const float*)m->pe, m->pe_rows, m->D, loop_step ? m->dy : (float*)nullptr));
-    MT3_LAUNCH_CHECK();
+    MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L,
+                              m->emb, m->pe, m->pe_rows, m->D, y_next, s));
   } else if (greedy) {
-    MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(m->B), dim3(256), 0, s, false, (const float*)logits, m->V, m->B,
-                                 use_finished ? m->tok_cur : (int*)nullptr, use_finished ? m->finished : (int*)nullptr,
-                                 tokens_ws, m->L, tok_user, m->state, 1, 0, (const float*)m->emb, (const float*)m->pe, m->pe_rows, m->D,
-                                 loop_step ? m->dy : (float*)nullptr));
-    MT3_LAUNCH_CHECK();
+    MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
+                               m->L, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D, y_next, m->B, s));
   } else {
     MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
     MT3_LAUNCH_CHECK();
@@ -897,13 +811,14 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
   m->att_scratch = (m->tc && enc_attention_tc_scratch_floats(batch, input_length, m->H) > 0) ? (float*)(b + w.att_scratch) : nullptr;
   m->dcounters_n = cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN);
   m->have_cross = false;
+  const bool s3 = m->split3;
+  m->a_h.hi = m->h; m->a_h.lo = s3 ? (float*)(b + w.h_lo) : nullptr;
+  m->a_ao.hi = m->ao; m->a_ao.lo = s3 ? (float*)(b + w.ao_lo) : nullptr;
+  m->a_g.hi = m->g; m->a_g.lo = s3 ? (float*)(b + w.g_lo) : nullptr;
+  m->a_qkv.hi = m->qkv; m->a_qkv.lo = s3 ? (float*)(b + w.qkv_lo) : nullptr;
   if (m->tc) {
     const int64_t M = (int64_t)batch * input_length;
-    const bool s3 = m->split3;
     m->a_x.hi = s3 ? (float*)(b + w.x_hi) : nullptr; m->a_x.lo = s3 ? (float*)(b + w.x_lo) : nullptr;
-    m->a_h.hi = m->h; m->a_h.lo = s3 ? (float*)(b + w.h_lo) : nullptr;
-    m->a_ao.hi = m->ao; m->a_ao.lo = s3 ? (float*)(b + w.ao_lo) : nullptr;
-    m->a_g.hi = m->g; m->a_g.lo = s3 ? (float*)(b + w.g_lo) : nullptr;
     m->a_enc.hi = s3 ? (float*)(b + w.enc_hi) : nullptr; m->a_enc.lo = s3 ? (float*)(b + w.enc_lo) : nullptr;
     if (s3) {
       MT3_TRY(make_operand(&m->a_x.op, m->a_x.hi, m->a_x.lo, M, m->cfg.input_depth, m->cfg.input_depth));
@@ -912,7 +827,6 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
     MT3_TRY(make_operand(&m->a_h.op, m->a_h.hi, m->a_h.lo, M, m->D, m->D));
     MT3_TRY(make_operand(&m->a_ao.op, m->a_ao.hi, m->a_ao.lo, M, m->Q, m->Q));
     MT3_TRY(make_operand(&m->a_g.op, m->a_g.hi, m->a_g.lo, M, m->F, m->F));
-    m->a_qkv.hi = m->qkv; m->a_qkv.lo = s3 ? (float*)(b + w.qkv_lo) : nullptr;
     MT3_TRY(make_operand(&m->a_qkv.op, m->a_qkv.hi, m->a_qkv.lo, M, 3 * m->Q, 3 * m->Q));
     m->a_vt.hi = (float*)(b + w.vt_hi); m->a_vt.lo = s3 ? (float*)(b + w.vt_lo) : nullptr;
     if (input_length % 4 == 0)   // TMA row pitch must be a multiple of 16 bytes; otherwise the SIMT attention kernel runs
@@ -1007,8 +921,7 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
     }
   }
   if (mode == 2) {
-    beam1_finalize_kernel<<<m->B, 128, 0, s>>>(m->tokens, m->B, m->L, ran, m->beam_i);
-    MT3_LAUNCH_CHECK();
+    MT3_TRY(launch_beam1_finalize(m->tokens, m->B, m->L, ran, m->beam_i, s));
   }
   MT3_CUDA_CHECK(cudaMemcpyAsync(tokens_out, m->tokens, (size_t)m->B * m->L * sizeof(int), cudaMemcpyDeviceToDevice, s));
   if (steps_run) *steps_run = ran;
@@ -1102,45 +1015,30 @@ extern "C" int mt3_debug_launch(mt3_model* h, int32_t kind, int32_t pos, int32_t
   MT3_NEED_WS(m);
   MT3_REQUIRE(pos >= 0 && pos < m->L && iters > 0, MT3_ERR_BAD_ARG, "mt3_debug_launch: bad pos/iters");
   cudaStream_t s = (cudaStream_t)stream;
-  const int B = m->B, D = m->D, Q = m->Q, L = m->L, T = m->T, M = B * T;
+  const int D = m->D, Q = m->Q, L = m->L, T = m->T;
   for (int it = 0; it < iters; ++it) {
     const int l = it % m->Ld;
     switch (kind) {
       case MT3_K_DEC_SELF_ATTN: {
-        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->skv, l, L), L, nullptr, pos + 1, m->dao, s));
+        MT3_TRY(dec_attention(m, m->dq, kv_layer(m, m->skv, l, L), L, nullptr, pos + 1, m->dao, s));
         break;
       }
       case MT3_K_DEC_CROSS_ATTN: {
-        MT3_TRY(launch_dec_attention(m, m->dq, kv_layer(m, m->ckv, l, T), T, nullptr, T, m->dao, s));
+        MT3_TRY(dec_attention(m, m->dq, kv_layer(m, m->ckv, l, T), T, nullptr, T, m->dao, s));
         break;
       }
       case MT3_K_DEC_QKV_GEMM: {
-        // scratch output: the encoder qkv buffer (B*T rows >= B)
-        MT3_TRY(dec_gemm(m, m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->qkv, 3 * Q, 3 * Q, nullptr, nullptr, s));
+        // scratch output: the encoder qkv buffer (B*T rows >= B).  Not the cache: after a full generate, *state is
+        // max_decode_length, and an append there would write past it.
+        MT3_TRY(dec_gemm(m, "gemm_qkv", m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->qkv, 3 * Q, 3 * Q, nullptr, nullptr, s));
         break;
       }
       case MT3_K_ENC_QKV_GEMM: {
-        if (m->tc) {
-          TcGemmArgs t = tc_args(M, 3 * Q, D, m->qkv, nullptr, 3 * Q);
-          t.row_scale = m->rstd;
-          MT3_TRY(launch_tc_gemm(m->a_h.op, m->enc[it % std::max(1, m->Le)].t_wqkv.op, t, m->split3, s));
-          break;
-        }
-        GemmArgs a = gemm_args(m->h, D, m->enc[it % std::max(1, m->Le)].wqkv, 3 * Q, M, 3 * Q, D, m->qkv, 3 * Q);
-        a.row_scale = m->rstd;
-        MT3_TRY(launch_sgemm(a, s));
+        MT3_TRY(enc_layer_qkv(m, it % std::max(1, m->Le), s));
         break;
       }
       case MT3_K_ENC_ATTN: {
-        if (m->tc && m->tc_attn_ok && enc_attention_tc_supported(T)) {
-          MT3_TRY(launch_enc_attention_tc(m->a_qkv.op, m->a_vt.op, B, T, m->H, m->a_ao.hi, m->a_ao.lo, m->split3, s, nullptr,
-                                          m->att_scratch));
-          break;
-        }
-        MT3_TRY(set_attr_once());
-        const size_t attn_smem = (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float);
-        enc_attention_kernel<<<dim3(cdiv(T, 32), m->H, B), 256, attn_smem, s>>>(m->qkv, 3 * Q, T, m->H, m->ao, nullptr, Q);
-        MT3_LAUNCH_CHECK();
+        MT3_TRY(enc_layer_attn(m, s));
         break;
       }
       default:

@@ -1,12 +1,11 @@
-"""Builds the standalone kernel bring-up binaries and the test-only kernel harness library
-(libmt3kernels.so, loaded by tests/test_kernel_parity.py and tests/test_decode_loop_kernels.py) next to this file (sm_90a).  A re-run is
-a no-op when every output is newer than the kernel sources."""
+"""Builds the test-only kernel harness library (libmt3kernels.so, loaded by tests/test_kernel_parity.py and
+tests/test_decode_loop_kernels.py) next to this file (sm_90a).  A re-run is a no-op when the library is newer than the
+kernel sources."""
 import os
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-TOOLS = ["gemm_tc_test", "attn_tc_test"]
 HARNESS = os.path.join(HERE, "libmt3kernels.so")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr"]
 
@@ -23,12 +22,6 @@ def harness_stale():
 
 def main():
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    for t in TOOLS:
-        src, out = os.path.join(HERE, t + ".cu"), os.path.join(HERE, t)
-        if not _stale(out, src):
-            continue
-        subprocess.run([nvcc, *FLAGS, "-o", out, src], check=True)
-        print("built", out)
     if harness_stale():
         subprocess.run([nvcc, *FLAGS, "-shared", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-o", HARNESS, os.path.join(HERE, "kernel_harness.cu")],
                        check=True)

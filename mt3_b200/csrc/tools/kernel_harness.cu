@@ -1,5 +1,6 @@
 // Test-only shared library (libmt3kernels.so): thin extern "C" launchers for the hot-path kernels, one kernel per call,
-// on caller-provided device pointers, on the legacy default stream.  tests/test_kernel_parity.py and
+// on caller-provided device pointers, on the legacy default stream.  Each calls the launcher the kernel's header defines
+// and model.cu uses, so grid, block, shared memory and attributes are the model's own.  tests/test_kernel_parity.py and
 // tests/test_decode_loop_kernels.py load it with ctypes and compare every kernel with a float64 (or exact) reference at
 // ragged shapes.  The argument structs (TcGemmArgs, GemmArgs, DecGemmArgs) are passed by pointer exactly as the kernels
 // take them, so every field is reachable from the tests; kh_sizeof() lets the caller check its mirror of their layout.  Every launcher returns an MT3_* status; kh_last_error()
@@ -53,24 +54,6 @@ __global__ void p24_roundtrip_kernel(const float* __restrict__ x, float* __restr
   }
 }
 
-template <int FMT>
-int launch_dec_attention_fmt(const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr, int len_add,
-                             int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim,
-                             float q_eps, int pf_tiles, int B) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(dec_attention_bulk_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr_done = true;
-  }
-  const size_t smem = dec_attention_smem(max_len);
-  MT3_REQUIRE(smem <= 100 * 1024, MT3_ERR_UNSUPPORTED, "decode attention: max_len %d too long", max_len);
-  MT3_CUDA_CHECK(launch_kernel(dec_attention_bulk_kernel<FMT, false>, dim3(H, B), dim3(kAttThreads), smem, (cudaStream_t)0, false,
-                               q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps,
-                               (unsigned long long*)nullptr, pf_tiles));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
-}
-
 }  // namespace
 
 #define KH_API __attribute__((visibility("default")))
@@ -107,20 +90,15 @@ KH_API int kh_enc_attention_tc(const float* qkv_hi, const float* qkv_lo, const f
   if (r != MT3_OK) return r;
   r = make_operand(&opv, vt_hi, vt_lo, (uint64_t)B * H * 64, (uint64_t)T, (uint64_t)T, 64);
   if (r != MT3_OK) return r;
-  return launch_enc_attention_tc(op, opv, B, T, H, out_hi, out_lo, split3 != 0, 0, nullptr, scratch);
+  return launch_enc_attention_tc(op, opv, B, T, H, out_hi, out_lo, split3 != 0, 0, scratch);
 }
 
 KH_API long long kh_enc_attention_tc_scratch_floats(int B, int T, int H) { return (long long)enc_attention_tc_scratch_floats(B, T, H); }
 KH_API int kh_enc_attention_tc_supported(int T) { return enc_attention_tc_supported(T) ? 1 : 0; }
 
-// the exact-fp32 encoder attention, launched as model.cu launches it
+// the exact-fp32 encoder attention
 KH_API int kh_enc_attention_fp32(const float* qkv, int B, int T, int H, float* out, float* out_lo) {
-  const size_t smem = (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float);
-  MT3_REQUIRE(smem <= 200 * 1024, MT3_ERR_UNSUPPORTED, "attention: T=%d too long", T);
-  MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  enc_attention_kernel<<<dim3(cdiv(T, 32), H, B), 256, smem>>>(qkv, 3 * H * 64, T, H, out, out_lo, H * 64);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_enc_attention(qkv, 3 * H * 64, T, H, B, out, out_lo, H * 64, 0);
 }
 
 KH_API int kh_dec_gemm_cluster(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, 0); }
@@ -130,12 +108,8 @@ KH_API int kh_dec_gemm_out_q(const DecGemmArgs* a0, const DecGemmArgs* a1) { ret
 KH_API int kh_dec_attention(int fmt, const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr, int len_add,
                      int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim, float q_eps,
                      int pf_tiles, int B) {
-  switch (fmt) {
-    case 0: return launch_dec_attention_fmt<0>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
-    case 1: return launch_dec_attention_fmt<1>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
-    case 2: return launch_dec_attention_fmt<2>(q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps, pf_tiles, B);
-    default: return fail(MT3_ERR_BAD_ARG, "decode attention: kv format %d", fmt);
-  }
+  return launch_dec_attention(fmt, q, ldq, q_off, kv, H, cap, len_ptr, len_add, max_len, out, ldo, q_ssq, q_ssq_n, q_ssq_ld, q_dim, q_eps,
+                              nullptr, pf_tiles, B, false, 0);
 }
 
 // n a multiple of 8; N = 1, 2 or 4 elements per kv_store call
@@ -149,50 +123,38 @@ KH_API int kh_p24_roundtrip(const float* x, float* y, uint32_t* code, long long 
   return MT3_OK;
 }
 
-// The decode loop's token pickers, embedding and the encoder's RMSNorm, launched with model.cu's grid and block sizes.
+// The decode loop's token pickers, embedding and the encoder's RMSNorm.
 // argmax_step_kernel: n_cta CTAs starting at sequence b0 (B spans the whole batch: the arrival counter advances the
 // position once all B sequences of the step have arrived, over however many launches).
 KH_API int kh_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* tok_user,
                           int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows, int D, float* y_next,
                           int n_cta) {
-  MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, (cudaStream_t)0, false, logits, V, B, tok_cur, finished,
-                               tokens_out, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows, D, y_next,
+                            n_cta, 0);
 }
 
 KH_API int kh_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
                          float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
                          float* y_next) {
-  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, (cudaStream_t)0, false, logits, V, B, tok_cur, finished,
-                               tokens_out, out_ld, state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, out_ld, state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D,
+                           y_next, 0);
 }
 
 KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i) {
-  beam1_finalize_kernel<<<B, 128>>>(tokens, B, L, steps, beam_i);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_beam1_finalize(tokens, B, L, steps, beam_i, 0);
 }
 
 // y [b0 + n, D] rows b0 .. b0 + n - 1
 KH_API int kh_embed(const int* tok, const float* emb, int D, int V, const float* pe, const int* pos_ptr, float* y, int b0, int n) {
-  MT3_CUDA_CHECK(launch_kernel(embed_kernel, dim3(n), dim3(128), 0, (cudaStream_t)0, false, tok, emb, D, V, pe, pos_ptr, y, b0));
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_embed(tok, emb, D, V, pe, pos_ptr, y, b0, n, 0);
 }
 
 KH_API int kh_row_rstd(const float* x, const float* x_lo, int ld, int M, int D, float eps, float* rstd) {
-  row_rstd_kernel<<<cdiv(M, 8), 256>>>(x, x_lo, ld, M, D, eps, rstd);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_row_rstd(x, x_lo, ld, M, D, eps, rstd, 0);
 }
 
 KH_API int kh_rmsnorm(const float* x, const float* x_lo, int ldx, int M, int D, float eps, const float* g, float* y, int ldy) {
-  rmsnorm_kernel<<<cdiv(M, 8), 256>>>(x, x_lo, ldx, M, D, eps, g, y, ldy);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
+  return launch_rmsnorm(x, x_lo, ldx, M, D, eps, g, y, ldy, 0);
 }
 
 }  // extern "C"
