@@ -24,6 +24,11 @@
 // Roofline: 655 360 algorithmic bytes and ~14.4 MFLOP of butterflies per mt3
 // segment; with hop 128 every sample feeds 16 frames, so the kernel is bound by
 // fp32 issue / shared memory, not HBM (DESIGN.md, "K1").
+// Range: every kernel here takes |X| of each bin other than DC and Nyquist as
+// sqrtf(Xr^2 + Xi^2), which is exact to rounding for about 2^-63 <= |X| <= 2^64.  Below,
+// Xr^2 + Xi^2 is subnormal and loses relative precision (under ~2^-75 it rounds to 0); above,
+// it overflows to +inf.  DC and Nyquist are real, |Z0.x +/- Z0.y|, and have neither limit;
+// nor do tf.abs and the float64 oracle.  Audio in [-1, 1] gives |X| <= N/2 <= 2^13.
 #include <math.h>
 #include <algorithm>
 #include <vector>
