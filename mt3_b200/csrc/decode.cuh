@@ -267,7 +267,7 @@ sgemm_dec_kernel(const DecGemmArgs p) {
 // No global scratch, no atomics, no second barrier (nobody reads remote memory after the barrier, so a CTA may exit
 // as soon as it is done).
 //
-// Arithmetic: exact fp32 FMA, k ascending (ffma2() in common.cuh).
+// Arithmetic: exact fp32 FMA, k ascending (ffma2() in common.cuh); with TC = true, 3xTF32 wgmma (dec_mma_3xtf32).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_map(uint32_t smem_addr, unsigned rank) {
   uint32_t r;
@@ -281,11 +281,96 @@ __device__ __forceinline__ void st_cluster_f1(uint32_t addr, float x) {
   asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(addr), "f"(x) : "memory");
 }
 
+__device__ __forceinline__ void st_cluster_f2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+
 constexpr int kDecLDB = kDecBN + 8;            // padded weight rows
 constexpr int kDecRedFloats = 8 * 8 * kDecBN;  // [src rank][local rows][32 cols] partials pushed to this CTA (S*R = 64 rows)
-template <int KC>
+// TC: the weight region holds the K-major tf32 hi and lo tiles (KC x 32 each) instead of the padded raw tile, plus room to
+// align them to 256 B
+template <int KC, bool TC>
 constexpr size_t dec_cluster_smem() {
-  return (size_t)(kDecBM * (KC + 4) + KC * kDecLDB + kDecRedFloats + 64) * sizeof(float);
+  return (size_t)(kDecBM * (KC + 4) + (TC ? 2 * KC * kDecBN + 64 : KC * kDecLDB) + kDecRedFloats + 64) * sizeof(float);
+}
+
+// The tensor-core multiply of the cluster kernel (gemm modes TF32X3 and TF32): D[64 x 32] = As[64 x KC] . W[KC x 32]
+// in 3xTF32 (gemm_tc.cuh: x = hi + lo, A.B ~= Alo.Bhi + Ahi.Blo + Ahi.Bhi, the lo.lo term dropped).
+//  B: cp.async leaves the weight tile row-major ([KC][32], unpadded) in the lo half of Bt; one pass through registers
+//     turns it into K-major hi and lo tiles (Bt, 256-B aligned; lo overwrites the raw tile) in the 32B-swizzle layout of
+//     smem_desc_k_sw32(): k-step j (8 k) is a column of four 8-row atoms at Bt + 1024 j, atom g holding columns
+//     8 g .. 8 g + 7.  A warp reads column n = lane and writes 4 consecutive k per 16-byte store: the swizzle spreads a
+//     quarter-warp's stores over all 32 banks.  The CTA needs no more shared memory than the FMA kernel's.
+//  A: fragments straight from As (wgmma_tf32_m64n64_rs layout), split in registers; with LDA = KC + 4 (= 4 or 20 mod
+//     32 words) the 8 rows x 4 columns a warp reads per register are 32 distinct banks.
+//  MMA: wgmma m64n32k8, A from registers, the two small terms into one accumulator and hi.hi into another (two
+//     independent chains instead of one of 3 KC / 8 dependent MMAs), summed at the end as hi.hi + (lo.hi + hi.lo).
+//     The k-steps go in groups of 2, one group in flight while the next one's fragments are loaded, so that only two
+//     groups of fragments hold registers (the kernel stays near 100 registers and leaves room on the SM for the
+//     attention kernel that starts under it).
+// d: the wgmma accumulator layout (tc.cuh): d[4j + 2h + {0, 1}] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + {0, 1}].
+template <int KC>
+__device__ __forceinline__ void dec_mma_3xtf32(const float* As, float* Bt, float (&d)[16]) {
+  constexpr int LDA = KC + 4, KS = KC / 8, BN = kDecBN;
+  static_assert(KS % 2 == 0, "k-steps go in pairs");
+  const int tid = threadIdx.x, w = tid / 32, l = tid % 32;
+  float* Bhi = Bt;
+  float* Blo = Bt + KC * BN;                   // holds the raw tile until the barrier below
+  {
+    const int n = l;
+    float4 raw[KC / 16];
+#pragma unroll
+    for (int i = 0; i < KC / 16; ++i) {
+      const int kq = w + 4 * i;
+      raw[i] = make_float4(Blo[(4 * kq + 0) * BN + n], Blo[(4 * kq + 1) * BN + n], Blo[(4 * kq + 2) * BN + n], Blo[(4 * kq + 3) * BN + n]);
+    }
+    __syncthreads();                           // every thread has read its part of the raw tile
+#pragma unroll
+    for (int i = 0; i < KC / 16; ++i) {
+      const int kq = w + 4 * i;
+      float4 h, lo;
+      split_tf32(raw[i].x, h.x, lo.x);
+      split_tf32(raw[i].y, h.y, lo.y);
+      split_tf32(raw[i].z, h.z, lo.z);
+      split_tf32(raw[i].w, h.w, lo.w);
+      const int off = (kq / 2) * 256 + (n / 8) * 64 + (n % 8) * 8 + (((kq & 1) ^ ((n >> 2) & 1)) * 4);
+      *reinterpret_cast<float4*>(Bhi + off) = h;
+      *reinterpret_cast<float4*>(Blo + off) = lo;
+    }
+  }
+  tc::fence_proxy_async();                     // the generic-proxy stores above -> visible to wgmma (async proxy)
+  __syncthreads();
+
+  const float* ar = As + (16 * w + l / 4) * LDA + l % 4;
+  const uint32_t bhi = tc::smem_u32(Bhi), blo = tc::smem_u32(Blo);
+  float small[16], big[16];
+#pragma unroll
+  for (int j0 = 0; j0 < KS; j0 += 2) {
+    uint32_t ah[2][4], al[2][4];
+#pragma unroll
+    for (int g = 0; g < 2; ++g)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {            // a0..a3: rows +0 / +8, columns +0 / +4 of k-step j0 + g
+        float hi, lo;
+        split_tf32(ar[(e & 1) * 8 * LDA + 8 * (j0 + g) + (e >> 1) * 4], hi, lo);
+        ah[g][e] = __float_as_uint(hi);
+        al[g][e] = __float_as_uint(lo);
+      }
+    tc::wgmma_fence();                       // this pair's fragment registers are written
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+      const int j = j0 + g;
+      const uint64_t dh = tc::smem_desc_k_sw32(bhi + j * 1024, 256), dl = tc::smem_desc_k_sw32(blo + j * 1024, 256);
+      tc::wgmma_tf32_m64n32_rs(small, al[g][0], al[g][1], al[g][2], al[g][3], dh, j > 0);
+      tc::wgmma_tf32_m64n32_rs(small, ah[g][0], ah[g][1], ah[g][2], ah[g][3], dl, true);
+      tc::wgmma_tf32_m64n32_rs(big, ah[g][0], ah[g][1], ah[g][2], ah[g][3], dh, j > 0);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();                     // the previous pair is done: its fragment registers are free
+  }
+  tc::wgmma_wait<0>();
+#pragma unroll
+  for (int i = 0; i < 16; ++i) d[i] = big[i] + small[i];
 }
 
 // Sum this rank's 64/S rows over the S source ranks (rank order, local shared memory) and apply the fused epilogue:
@@ -341,17 +426,21 @@ __device__ __forceinline__ void dec_reduce_epilogue(const DecGemmArgs& p, const 
   }
 }
 
-// One warp group (128 threads) per CTA: the multiply loop is bound by shared-memory bandwidth (8 LDS.128 per 64 FMAs
-// with 4 x 4 register tiles), not by issue latency, so more warps would only add a step that combines their partials.
-template <int KC, bool TRACE, int S>
+// One warp group (128 threads) per CTA: the SIMT multiply loop is bound by shared-memory bandwidth (8 LDS.128 per 64
+// FMAs with 4 x 4 register tiles), not by issue latency, so more warps would only add a step that combines their
+// partials.  TC: the multiply runs on the tensor cores instead (dec_mma_3xtf32); loads, the RMSNorm statistic, the
+// exchange, the reduction order and the epilogue are the same.
+template <int KC, bool TRACE, int S, bool TC>
 __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x, const KvStage& kst) {
-  constexpr int BM = kDecBM, BN = kDecBN, NT = 128, LDA = KC + 4, LDB = kDecLDB;
+  constexpr int BM = kDecBM, BN = kDecBN, NT = 128, LDA = KC + 4, LDB = TC ? kDecBN : kDecLDB;
   constexpr int R = BM / S;                   // rows of the tile each rank owns (8 for clusters of 8, 4 for clusters of 16)
   static_assert(KC % 8 == 0, "K chunk must split into float4 pieces per ssq thread");
   extern __shared__ __align__(16) float dsm[];
   float* As = dsm;                            // [BM][LDA] activations, row-major
-  float* Bs = As + BM * LDA;                  // [KC][LDB] weights
-  float* Red = Bs + KC * LDB;                 // [S src][R rows][BN] partial tiles of MY rows (written by all ranks)
+  // TC: Bt = the hi / lo tiles of dec_mma_3xtf32 (256-B aligned), the raw weights land in its lo half
+  float* Bt = TC ? As + BM * LDA + (((tc::smem_u32(As + BM * LDA) + 255u) & ~255u) - tc::smem_u32(As + BM * LDA)) / 4 : nullptr;
+  float* Bs = TC ? Bt + KC * BN : As + BM * LDA;   // [KC][LDB] weights
+  float* Red = TC ? As + BM * LDA + 2 * KC * BN + 64 : Bs + KC * LDB;   // [S src][R rows][BN] partial tiles of MY rows (written by all ranks)
   float* Rss = Red + kDecRedFloats;           // [S src][R rows] partial sums of squares of my rows
 
   unsigned rank;
@@ -417,22 +506,27 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
   // ascending ----
   const int tx = threadIdx.x % 8, ty = threadIdx.x / 8;           // unsigned: shifts without a sign fix-up
   float2 acc[4][2];
+  float d[16];                                                     // TC: the wgmma accumulator layout
+  if constexpr (TC) {
+    dec_mma_3xtf32<KC>(As, Bt, d);
+  } else {
 #pragma unroll
-  for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = make_float2(0.f, 0.f);
+    for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = make_float2(0.f, 0.f);
 #pragma unroll 4
-  for (int k = 0; k < KC; k += 4) {
-    float4 a[4], b[4];
+    for (int k = 0; k < KC; k += 4) {
+      float4 a[4], b[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(&As[(ty + 16 * i) * LDA + k]);
+      for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(&As[(ty + 16 * i) * LDA + k]);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) b[kk] = *reinterpret_cast<const float4*>(&Bs[(k + kk) * LDB + tx * 4]);
+      for (int kk = 0; kk < 4; ++kk) b[kk] = *reinterpret_cast<const float4*>(&Bs[(k + kk) * LDB + tx * 4]);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
+      for (int i = 0; i < 4; ++i) {
+        const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        ffma2(acc[i][0], av[kk], make_float2(b[kk].x, b[kk].y));
-        ffma2(acc[i][1], av[kk], make_float2(b[kk].z, b[kk].w));
+        for (int kk = 0; kk < 4; ++kk) {
+          ffma2(acc[i][0], av[kk], make_float2(b[kk].x, b[kk].y));
+          ffma2(acc[i][1], av[kk], make_float2(b[kk].z, b[kk].w));
+        }
       }
     }
   }
@@ -441,11 +535,22 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
 
   const uint32_t red_base = tc::smem_u32(Red) + rank * (R * BN * 4);     // my slot [rank][..] in the owner's Red
   const uint32_t rss_base = tc::smem_u32(Rss) + rank * (R * 4);
+  if constexpr (TC) {
+    const int w = tid / 32, l = tid % 32;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {                                    // row ty + 16 i -> owner rank, local row
-    const int row = ty + 16 * i;
-    st_cluster_f4(cluster_map(red_base + (uint32_t)(((row % R) * BN + tx * 4) * 4), (unsigned)(row / R)),
-                  make_float4(acc[i][0].x, acc[i][0].y, acc[i][1].x, acc[i][1].y));
+    for (int h = 0; h < 2; ++h) {                                  // rows 16 w + l / 4 (+ 8) -> owner rank, local row
+      const int row = 16 * w + l / 4 + 8 * h;
+      const uint32_t dst = cluster_map(red_base + (uint32_t)(((row % R) * BN + 2 * (l % 4)) * 4), (unsigned)(row / R));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) st_cluster_f2(dst + 32 * j, d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {                                  // row ty + 16 i -> owner rank, local row
+      const int row = ty + 16 * i;
+      st_cluster_f4(cluster_map(red_base + (uint32_t)(((row % R) * BN + tx * 4) * 4), (unsigned)(row / R)),
+                    make_float4(acc[i][0].x, acc[i][0].y, acc[i][1].x, acc[i][1].y));
+    }
   }
   if (p.norm && (tid % 2) == 0) {
     const int row = tid / 2;
@@ -461,79 +566,90 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
   }
 }
 
-template <int KC, bool TRACE, int S>
+template <int KC, bool TRACE, int S, bool TC>
 __global__ void __launch_bounds__(128)
 sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst) {
-  dec_cluster_body<KC, TRACE, S>(p, (int)blockIdx.x, kst);
+  dec_cluster_body<KC, TRACE, S, TC>(p, (int)blockIdx.x, kst);
 }
 
 // Two independent GEMMs that read the same inputs in ONE launch (column tiles [0, tiles0) belong to p0, the rest to
 // p1): used for  y' = y + o.Wo  together with  q_raw = [o | y].[Wo.Wq ; Wq]  (the out-projection folded into the
 // next projection with a precomposed weight block), which removes a kernel from the dependency chain.
-template <int KC0, int KC1, bool TRACE>
+template <int KC0, int KC1, bool TRACE, bool TC>
 __global__ void __launch_bounds__(128)
 sgemm_dec_cluster2_kernel(const DecGemmArgs p0, const DecGemmArgs p1, const int tiles0) {
-  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8>(p0, (int)blockIdx.x, KvStage{});
-  else dec_cluster_body<KC1, TRACE, 8>(p1, (int)blockIdx.x - tiles0, KvStage{});
+  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, TC>(p0, (int)blockIdx.x, KvStage{});
+  else dec_cluster_body<KC1, TRACE, 8, TC>(p1, (int)blockIdx.x - tiles0, KvStage{});
 }
 
-// the mt3 shapes: K = 384 (out-projection) and K = 384 + 512 (precomposed query block); MT3_ERR_UNSUPPORTED (without
-// launching) for any other
-inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, cudaStream_t s) {
+template <bool TC>
+inline int launch_dec_gemm_out_q_tc(const DecGemmArgs& a0, const DecGemmArgs& a1, cudaStream_t s) {
   constexpr int KC0 = 48, KC1 = 112;
-  if (a0.M > kDecBM || a1.M > kDecBM || a0.K != 8 * KC0 || a1.K != 8 * KC1 || a0.N % kDecBN != 0 || a1.N % kDecBN != 0)
-    return MT3_ERR_UNSUPPORTED;
-  constexpr size_t smem = dec_cluster_smem<KC1>();
+  constexpr size_t smem = dec_cluster_smem<KC1, TC>();
   static bool attr_done = false;
   if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
   const int tiles0 = a0.N / kDecBN, tiles1 = a1.N / kDecBN;
   if (a0.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
                                          a0, a1, tiles0));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
                                          a0, a1, tiles0));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
-template <int KC, int S>
+// the mt3 shapes: K = 384 (out-projection) and K = 384 + 512 (precomposed query block); MT3_ERR_UNSUPPORTED (without
+// launching) for any other.  tc: the 3xTF32 tensor-core multiply (dec_mma_3xtf32), else exact fp32.
+inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, bool tc, cudaStream_t s) {
+  if (a0.M > kDecBM || a1.M > kDecBM || a0.K != 8 * 48 || a1.K != 8 * 112 || a0.N % kDecBN != 0 || a1.N % kDecBN != 0)
+    return MT3_ERR_UNSUPPORTED;
+  return tc ? launch_dec_gemm_out_q_tc<true>(a0, a1, s) : launch_dec_gemm_out_q_tc<false>(a0, a1, s);
+}
+
+template <int KC, int S, bool TC>
 inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst) {
-  constexpr size_t smem = dec_cluster_smem<KC>();
+  constexpr size_t smem = dec_cluster_smem<KC, TC>();
   static bool attr_done = false;
   if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (S > 8) {
-      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, TC>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, TC>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     }
     attr_done = true;
   }
   if (a.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
-// Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.
-inline int launch_dec_gemm_cluster(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst = KvStage{}) {
-  if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
+template <bool TC>
+inline int launch_dec_gemm_cluster_tc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst) {
   // the long-K, narrow-N GEMM (MLP out: K = 1024, N = 512) has only N/32 x 8 = 128 CTAs at cluster size 8: a
   // cluster of 16 halves every CTA's K chunk and fills the machine
-  if (a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16>(a, s, kst);
+  if (a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, TC>(a, s, kst);
   switch (a.K / 8) {
-    case 48: return launch_dec_gemm_cluster_kc<48, 8>(a, s, kst);
-    case 64: return launch_dec_gemm_cluster_kc<64, 8>(a, s, kst);
-    case 128: return launch_dec_gemm_cluster_kc<128, 8>(a, s, kst);
+    case 48: return launch_dec_gemm_cluster_kc<48, 8, TC>(a, s, kst);
+    case 64: return launch_dec_gemm_cluster_kc<64, 8, TC>(a, s, kst);
+    case 128: return launch_dec_gemm_cluster_kc<128, 8, TC>(a, s, kst);
     default: return MT3_ERR_UNSUPPORTED;
   }
+}
+
+// Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.  tc: the 3xTF32
+// tensor-core multiply (dec_mma_3xtf32), else exact fp32.
+inline int launch_dec_gemm_cluster(const DecGemmArgs& a, bool tc, cudaStream_t s, const KvStage& kst = KvStage{}) {
+  if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
+  return tc ? launch_dec_gemm_cluster_tc<true>(a, s, kst) : launch_dec_gemm_cluster_tc<false>(a, s, kst);
 }
 
 inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s) {

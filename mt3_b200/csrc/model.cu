@@ -331,8 +331,9 @@ static unsigned long long* trace_slot(Model* m, const char* name) {
   return m->trace + (size_t)(m->trace_names.size() - 1) * kTraceWords;
 }
 
-// Decode-step GEMM on M = B rows in blocks of 64: split-K exact-fp32 cluster kernel with the RMSNorm statistic fused
-// (decode.cuh), in every gemm_mode; the non-cluster kernel for K the cluster kernel does not tile.
+// Decode-step GEMM on M = B rows in blocks of 64: split-K cluster kernel with the RMSNorm statistic fused (decode.cuh);
+// its multiply is exact fp32 in gemm_mode SIMT and 3xTF32 on the tensor cores in both tensor modes (single-pass TF32
+// stays an encoder-only trade).  The non-cluster kernel (exact fp32) for K the cluster kernel does not tile.
 // name: the node's trace name (mt3_debug_trace_step).
 static int dec_gemm(Model* m, const char* name, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C,
                     int ldc, int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{}) {
@@ -351,7 +352,7 @@ static int dec_gemm(Model* m, const char* name, const float* A, int lda, const f
     a.partial = m->dpartial;
     a.counters = m->dcounters;
     a.trace = trace_slot(m, name);
-    int rc = launch_dec_gemm_cluster(a, s, r0 == 0 ? kst : KvStage{});
+    int rc = launch_dec_gemm_cluster(a, m->tc, s, r0 == 0 ? kst : KvStage{});
     if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s);
     MT3_TRY(rc);
   }
@@ -384,7 +385,7 @@ static int dec_gemm_out_q(Model* m, const DecLayer& w, const float* y_in, float*
   a1.eps = 1e-6f; a1.epi = EPI_STORE; a1.C = m->dq; a1.ldc = Q; a1.n_split = Q;
   a1.R = a1.C; a1.ldr = Q;
   a1.trace = a0.trace;
-  return launch_dec_gemm_out_q(a0, a1, s);
+  return launch_dec_gemm_out_q(a0, a1, m->tc, s);
 }
 
 // The state one decode step carries from layer to layer: the current residual-stream buffer (ping-pongs between m->dy

@@ -99,6 +99,18 @@ __device__ __forceinline__ void wgmma_tf32_m64n64_rs(float (&d)[32], uint32_t a0
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc)
       : "memory");
 }
+// D[64 x 32] (+)= A[64 x 8] . B[32 x 8]^T with the A operand in registers (fragment as for m64n64 above); accumulate =
+// false: D = A . B (the accumulator's old contents are not read).
+__device__ __forceinline__ void wgmma_tf32_m64n32_rs(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc,
+                                                     bool accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"((int)accumulate)
+      : "memory");
+}
 
 // ---- descriptors ------------------------------------------------------------------------
 // Shared-memory matrix descriptor (64 bit), K-major operand stored as 128-byte rows with the
@@ -113,6 +125,21 @@ __device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
   d |= (uint64_t)1 << 62;
+  return d;
+}
+
+// The same for a K-major operand stored as 32-byte rows with the 32B swizzle (8-row x 32 B atoms: row r of an atom at
+// byte 32 r, its two 16-byte halves swapped when r & 4).  One atom holds one k-step of 8 tf32 for 8 rows, so a
+// k-step's operand is a column of atoms and the next k-step starts at a new address (no in-row advance):
+//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (unused: K per wgmma = the 32 B row; 1)
+//   [32,46) stride byte offset >> 4   = sbo >> 4 (distance between 8-row atoms)
+//   [49,52) base offset = 0 (atoms are 256-B aligned)   [62,64) layout type: 3 = SWIZZLE_32B
+__device__ __forceinline__ uint64_t smem_desc_k_sw32(uint32_t smem_addr, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(sbo >> 4) << 32;
+  d |= (uint64_t)3 << 62;
   return d;
 }
 

@@ -101,9 +101,12 @@ KH_API int kh_enc_attention_fp32(const float* qkv, int B, int T, int H, float* o
   return launch_enc_attention(qkv, 3 * H * 64, T, H, B, out, out_lo, H * 64, 0);
 }
 
-KH_API int kh_dec_gemm_cluster(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, 0); }
+KH_API int kh_dec_gemm_cluster(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, false, 0); }
 KH_API int kh_dec_gemm(const DecGemmArgs* a) { return launch_dec_gemm(*a, 0); }
-KH_API int kh_dec_gemm_out_q(const DecGemmArgs* a0, const DecGemmArgs* a1) { return launch_dec_gemm_out_q(*a0, *a1, 0); }
+KH_API int kh_dec_gemm_out_q(const DecGemmArgs* a0, const DecGemmArgs* a1) { return launch_dec_gemm_out_q(*a0, *a1, false, 0); }
+// the same launches with the 3xTF32 tensor-core multiply (the decoder's path in gemm modes TF32X3 and TF32)
+KH_API int kh_dec_gemm_cluster_tc(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, true, 0); }
+KH_API int kh_dec_gemm_out_q_tc(const DecGemmArgs* a0, const DecGemmArgs* a1) { return launch_dec_gemm_out_q(*a0, *a1, true, 0); }
 
 KH_API int kh_dec_attention(int fmt, const float* q, int ldq, int q_off, const void* kv, int H, int cap, const int* len_ptr, int len_add,
                      int max_len, float* out, int ldo, const float* q_ssq, int q_ssq_n, int q_ssq_ld, float q_dim, float q_eps,
