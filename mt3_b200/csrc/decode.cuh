@@ -84,7 +84,21 @@ struct DecGemmArgs {
   // output sums the N/32 partials in order and gets the RMSNorm statistic without re-reading the row
   float* ssq_out; int ssq_ld;
   unsigned long long* trace;      // debug timeline slot (mt3_debug_trace_step) or null: [0] min start, [1] max end (ns,
-                                  // %globaltimer); [2..6] clock64 deltas of CTA (0,0) at its phase boundaries
+                                  // %globaltimer); [2..7] clock64 deltas of CTA (0,0) at its phase boundaries
+};
+
+// How a cluster-kernel launch is chained to its neighbours in the stream by programmatic dependent launch (PDL).
+//  pdl: the launch is a programmatic dependent of the preceding GEMM node: its CTAs may start while that node still runs
+//       and load their weight tiles under it.  Before griddepcontrol.wait a CTA issues only weight loads and sets up its
+//       cluster barrier.
+//  late_trigger: each CTA lets the dependent grid launch after the cluster exchange instead of right after the wait.  An
+//       attention kernel as the successor wants the early trigger: it streams K/V rows no decode GEMM writes and gains
+//       from every microsecond it starts sooner.  A PDL-launched GEMM as the successor loads weights from HBM; where this
+//       node streams 2.4-4 MB of weights itself (MLP-in, MLP-out) those loads compete with its load phase, and the late
+//       trigger overlaps them with its reduction, its epilogue and the launch gap instead (DESIGN.md §3).
+struct DecChain {
+  bool pdl = false;
+  bool late_trigger = false;
 };
 
 __device__ __forceinline__ unsigned long long gtime_ns() {
@@ -309,38 +323,45 @@ constexpr size_t dec_cluster_smem() {
 //     groups of fragments hold registers (the kernel stays near 100 registers and leaves room on the SM for the
 //     attention kernel that starts under it).
 // d: the wgmma accumulator layout (tc.cuh): d[4j + 2h + {0, 1}] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + {0, 1}].
+// dec_split_weights turns the landed raw tile into the hi / lo tiles; it needs only the weights, so it runs while the
+// activations are still in flight.  dec_mma_3xtf32 then multiplies.
 template <int KC>
-__device__ __forceinline__ void dec_mma_3xtf32(const float* As, float* Bt, float (&d)[16]) {
-  constexpr int LDA = KC + 4, KS = KC / 8, BN = kDecBN;
-  static_assert(KS % 2 == 0, "k-steps go in pairs");
+__device__ __forceinline__ void dec_split_weights(float* Bt) {
+  constexpr int BN = kDecBN;
   const int tid = threadIdx.x, w = tid / 32, l = tid % 32;
   float* Bhi = Bt;
   float* Blo = Bt + KC * BN;                   // holds the raw tile until the barrier below
-  {
-    const int n = l;
-    float4 raw[KC / 16];
+  const int n = l;
+  float4 raw[KC / 16];
 #pragma unroll
-    for (int i = 0; i < KC / 16; ++i) {
-      const int kq = w + 4 * i;
-      raw[i] = make_float4(Blo[(4 * kq + 0) * BN + n], Blo[(4 * kq + 1) * BN + n], Blo[(4 * kq + 2) * BN + n], Blo[(4 * kq + 3) * BN + n]);
-    }
-    __syncthreads();                           // every thread has read its part of the raw tile
+  for (int i = 0; i < KC / 16; ++i) {
+    const int kq = w + 4 * i;
+    raw[i] = make_float4(Blo[(4 * kq + 0) * BN + n], Blo[(4 * kq + 1) * BN + n], Blo[(4 * kq + 2) * BN + n], Blo[(4 * kq + 3) * BN + n]);
+  }
+  __syncthreads();                             // every thread has read its part of the raw tile
 #pragma unroll
-    for (int i = 0; i < KC / 16; ++i) {
-      const int kq = w + 4 * i;
-      float4 h, lo;
-      split_tf32(raw[i].x, h.x, lo.x);
-      split_tf32(raw[i].y, h.y, lo.y);
-      split_tf32(raw[i].z, h.z, lo.z);
-      split_tf32(raw[i].w, h.w, lo.w);
-      const int off = (kq / 2) * 256 + (n / 8) * 64 + (n % 8) * 8 + (((kq & 1) ^ ((n >> 2) & 1)) * 4);
-      *reinterpret_cast<float4*>(Bhi + off) = h;
-      *reinterpret_cast<float4*>(Blo + off) = lo;
-    }
+  for (int i = 0; i < KC / 16; ++i) {
+    const int kq = w + 4 * i;
+    float4 h, lo;
+    split_tf32(raw[i].x, h.x, lo.x);
+    split_tf32(raw[i].y, h.y, lo.y);
+    split_tf32(raw[i].z, h.z, lo.z);
+    split_tf32(raw[i].w, h.w, lo.w);
+    const int off = (kq / 2) * 256 + (n / 8) * 64 + (n % 8) * 8 + (((kq & 1) ^ ((n >> 2) & 1)) * 4);
+    *reinterpret_cast<float4*>(Bhi + off) = h;
+    *reinterpret_cast<float4*>(Blo + off) = lo;
   }
   tc::fence_proxy_async();                     // the generic-proxy stores above -> visible to wgmma (async proxy)
   __syncthreads();
+}
 
+template <int KC>
+__device__ __forceinline__ void dec_mma_3xtf32(const float* As, const float* Bt, float (&d)[16]) {
+  constexpr int LDA = KC + 4, KS = KC / 8, BN = kDecBN;
+  static_assert(KS % 2 == 0, "k-steps go in pairs");
+  const int tid = threadIdx.x, w = tid / 32, l = tid % 32;
+  const float* Bhi = Bt;
+  const float* Blo = Bt + KC * BN;
   const float* ar = As + (16 * w + l / 4) * LDA + l % 4;
   const uint32_t bhi = tc::smem_u32(Bhi), blo = tc::smem_u32(Blo);
   float small[16], big[16];
@@ -431,7 +452,7 @@ __device__ __forceinline__ void dec_reduce_epilogue(const DecGemmArgs& p, const 
 // partials.  TC: the multiply runs on the tensor cores instead (dec_mma_3xtf32); loads, the RMSNorm statistic, the
 // exchange, the reduction order and the epilogue are the same.
 template <int KC, bool TRACE, int S, bool TC>
-__device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x, const KvStage& kst) {
+__device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int tile_x, const KvStage& kst, const DecChain& ch) {
   constexpr int BM = kDecBM, BN = kDecBN, NT = 128, LDA = KC + 4, LDB = TC ? kDecBN : kDecLDB;
   constexpr int R = BM / S;                   // rows of the tile each rank owns (8 for clusters of 8, 4 for clusters of 16)
   static_assert(KC % 8 == 0, "K chunk must split into float4 pieces per ssq thread");
@@ -463,9 +484,12 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
   // "I am running": peers may write into my shared memory once every CTA of the cluster has arrived here
   asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
 
-  // ---- load phase: cp.async (global -> shared, no register staging): all of the CTA's weights and activations
-  // are in flight at once; one wait.  Weights are issued BEFORE the PDL wait (they do not depend on the
-  // previous kernel).
+  // ---- load phase: cp.async (global -> shared, no register staging), weights and activations as two commit groups.
+  // Weights are issued BEFORE the PDL wait (they do not depend on the previous kernel): a CTA that starts under the
+  // preceding GEMM node has them by the time the wait returns.  In the tensor modes the weight tile is split into its hi /
+  // lo tiles while the activations are in flight.  (Splitting before the wait as well was slower: a CTA that cannot
+  // start early, such as the MLP-out clusters that do not fit beside the MLP-in, then loads weights, splits and loads
+  // activations one after the other; DESIGN.md §3.)
   for (int idx = tid; idx < KC * 8; idx += NT) {
     const int kr = idx >> 3, nq = idx & 7;
     const bool ok = n0 + nq * 4 < p.N;
@@ -473,8 +497,10 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(tc::smem_u32(&Bs[kr * LDB + nq * 4])), "l"(src),
                  "r"(ok ? 16 : 0) : "memory");
   }
+  asm volatile("cp.async.commit_group;" ::: "memory");
   pdl_wait();
-  pdl_trigger();
+  if (tr0) p.trace[6] = (unsigned long long)(clock64() - c0);      // wait returned
+  if (!ch.late_trigger) pdl_trigger();
   for (int idx = tid; idx < KC * 16; idx += NT) {
     const int row = idx / (KC / 4), kq = idx % (KC / 4);
     const bool ok = row < p.M;
@@ -485,7 +511,14 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
                  "r"(ok ? 16 : 0) : "memory");
   }
   if (tid == 0) l2_stage_kv(kst, blockIdx.y * gridDim.x + blockIdx.x, gridDim.x * gridDim.y);
-  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+  asm volatile("cp.async.commit_group;" ::: "memory");
+  if constexpr (TC) {
+    asm volatile("cp.async.wait_group 1;" ::: "memory");
+    __syncthreads();
+    dec_split_weights<KC>(Bt);
+    if (tr0) p.trace[7] = (unsigned long long)(clock64() - c0);    // weights landed and split
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   if (tr0) p.trace[2] = (unsigned long long)(clock64() - c0);      // loads landed
 
@@ -558,6 +591,7 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
   }
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
   if (tr0) p.trace[4] = (unsigned long long)(clock64() - c0);      // partials exchanged
+  if (ch.late_trigger) pdl_trigger();
 
   dec_reduce_epilogue<S>(p, Red, Rss, rank, n0);
   if (tr) {
@@ -568,8 +602,8 @@ __device__ __forceinline__ void dec_cluster_body(const DecGemmArgs& p, const int
 
 template <int KC, bool TRACE, int S, bool TC>
 __global__ void __launch_bounds__(128)
-sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst) {
-  dec_cluster_body<KC, TRACE, S, TC>(p, (int)blockIdx.x, kst);
+sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst, const DecChain ch) {
+  dec_cluster_body<KC, TRACE, S, TC>(p, (int)blockIdx.x, kst, ch);
 }
 
 // Two independent GEMMs that read the same inputs in ONE launch (column tiles [0, tiles0) belong to p0, the rest to
@@ -578,8 +612,9 @@ sgemm_dec_cluster_kernel(const DecGemmArgs p, const KvStage kst) {
 template <int KC0, int KC1, bool TRACE, bool TC>
 __global__ void __launch_bounds__(128)
 sgemm_dec_cluster2_kernel(const DecGemmArgs p0, const DecGemmArgs p1, const int tiles0) {
-  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, TC>(p0, (int)blockIdx.x, KvStage{});
-  else dec_cluster_body<KC1, TRACE, 8, TC>(p1, (int)blockIdx.x - tiles0, KvStage{});
+  // runs between two attention kernels: not PDL-launched, triggers the cross-attention right after its wait
+  if ((int)blockIdx.x < tiles0) dec_cluster_body<KC0, TRACE, 8, TC>(p0, (int)blockIdx.x, KvStage{}, DecChain{});
+  else dec_cluster_body<KC1, TRACE, 8, TC>(p1, (int)blockIdx.x - tiles0, KvStage{}, DecChain{});
 }
 
 template <bool TC>
@@ -590,14 +625,18 @@ inline int launch_dec_gemm_out_q_tc(const DecGemmArgs& a0, const DecGemmArgs& a1
   if (!attr_done) {
     MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                        cudaSharedmemCarveoutMaxShared));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                        cudaSharedmemCarveoutMaxShared));
     attr_done = true;
   }
   const int tiles0 = a0.N / kDecBN, tiles1 = a1.N / kDecBN;
   if (a0.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, true, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u, false,
                                          a0, a1, tiles0));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u,
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster2_kernel<KC0, KC1, false, TC>, dim3(tiles0 + tiles1, 8), dim3(128), smem, s, 8u, false,
                                          a0, a1, tiles0));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
@@ -612,7 +651,7 @@ inline int launch_dec_gemm_out_q(const DecGemmArgs& a0, const DecGemmArgs& a1, b
 }
 
 template <int KC, int S, bool TC>
-inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst) {
+inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst, const DecChain& ch) {
   constexpr size_t smem = dec_cluster_smem<KC, TC>();
   static bool attr_done = false;
   if (!attr_done) {
@@ -622,34 +661,42 @@ inline int launch_dec_gemm_cluster_kc(const DecGemmArgs& a, cudaStream_t s, cons
       MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, TC>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
       MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, TC>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     }
+    // every decode GEMM asks for the largest shared-memory carveout: an SM only takes CTAs of a grid whose carveout matches
+    // its current one, so without this the CTAs of a PDL-launched GEMM could not start beside those of a GEMM with a
+    // smaller footprint (the cross out-projection at KC 48) and waited for the SMs to drain
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, false, S, TC>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                        cudaSharedmemCarveoutMaxShared));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(sgemm_dec_cluster_kernel<KC, true, S, TC>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                        cudaSharedmemCarveoutMaxShared));
     attr_done = true;
   }
   if (a.trace)
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, true, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, ch.pdl, a, kst, ch));
   else
-    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, a, kst));
+    MT3_CUDA_CHECK(launch_kernel_cluster(sgemm_dec_cluster_kernel<KC, false, S, TC>, dim3(cdiv(a.N, kDecBN), S), dim3(128), smem, s, (unsigned)S, ch.pdl, a, kst, ch));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
 template <bool TC>
-inline int launch_dec_gemm_cluster_tc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst) {
+inline int launch_dec_gemm_cluster_tc(const DecGemmArgs& a, cudaStream_t s, const KvStage& kst, const DecChain& ch) {
   // the long-K, narrow-N GEMM (MLP out: K = 1024, N = 512) has only N/32 x 8 = 128 CTAs at cluster size 8: a
   // cluster of 16 halves every CTA's K chunk and fills the machine
-  if (a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, TC>(a, s, kst);
+  if (a.K == 1024 && a.epi != EPI_GATED_GELU && a.N <= 512) return launch_dec_gemm_cluster_kc<64, 16, TC>(a, s, kst, ch);
   switch (a.K / 8) {
-    case 48: return launch_dec_gemm_cluster_kc<48, 8, TC>(a, s, kst);
-    case 64: return launch_dec_gemm_cluster_kc<64, 8, TC>(a, s, kst);
-    case 128: return launch_dec_gemm_cluster_kc<128, 8, TC>(a, s, kst);
+    case 48: return launch_dec_gemm_cluster_kc<48, 8, TC>(a, s, kst, ch);
+    case 64: return launch_dec_gemm_cluster_kc<64, 8, TC>(a, s, kst, ch);
+    case 128: return launch_dec_gemm_cluster_kc<128, 8, TC>(a, s, kst, ch);
     default: return MT3_ERR_UNSUPPORTED;
   }
 }
 
 // Returns MT3_ERR_UNSUPPORTED (without launching) when K does not split into 8 chunks of 48/64/128.  tc: the 3xTF32
-// tensor-core multiply (dec_mma_3xtf32), else exact fp32.
-inline int launch_dec_gemm_cluster(const DecGemmArgs& a, bool tc, cudaStream_t s, const KvStage& kst = KvStage{}) {
+// tensor-core multiply (dec_mma_3xtf32), else exact fp32.  ch: PDL edge into the launch and trigger placement (DecChain).
+inline int launch_dec_gemm_cluster(const DecGemmArgs& a, bool tc, cudaStream_t s, const KvStage& kst = KvStage{},
+                                   const DecChain& ch = DecChain{}) {
   if (a.M > kDecBM || a.N % 4 != 0 || a.lda % 4 != 0 || a.ldw % 4 != 0 || a.n_split % 4 != 0 || a.K % 8 != 0) return MT3_ERR_UNSUPPORTED;
-  return tc ? launch_dec_gemm_cluster_tc<true>(a, s, kst) : launch_dec_gemm_cluster_tc<false>(a, s, kst);
+  return tc ? launch_dec_gemm_cluster_tc<true>(a, s, kst, ch) : launch_dec_gemm_cluster_tc<false>(a, s, kst, ch);
 }
 
 inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s) {
@@ -657,6 +704,7 @@ inline int launch_dec_gemm(const DecGemmArgs& a, cudaStream_t s) {
   MT3_REQUIRE(a.K % kDecKC == 0 && a.K / kDecKC <= 16 && a.N % 4 == 0 && a.lda % 4 == 0 && a.ldw % 4 == 0 && a.n_split % 4 == 0,
               MT3_ERR_UNSUPPORTED, "decode gemm: K=%d must be a multiple of %d (at most 16 chunks); N=%d", a.K, kDecKC, a.N);
   MT3_REQUIRE(a.A2 == nullptr, MT3_ERR_UNSUPPORTED, "decode gemm: the two-source form needs the cluster kernel");
+  // never PDL-launched: it shares the partial / counters scratch with every other node that takes this kernel
   MT3_CUDA_CHECK(launch_kernel(sgemm_dec_kernel, dim3(cdiv(a.N, kDecBN), a.K / kDecKC), dim3(128), 0, s, false, a));
   MT3_LAUNCH_CHECK();
   return MT3_OK;

@@ -97,6 +97,8 @@ struct Model {
                                   // 0 = off)
   int pf_kv = 4;        // MT3_PF_KV=n: the GEMM node before each layer's QKV projection prefetches the first n tiles of every
                                   // K and V stream of that layer's self-attention into L2 (decode.cuh KvStage; value-neutral; 0 = off)
+  bool pdl_gemm = true;           // programmatic edges between consecutive decode GEMM nodes (dec_chain()); MT3_PDL_GEMM=0 turns
+                                  // them off, the reference for the value-neutrality tests
   int kv_fmt = 0;                 // cfg.kv_cache_format: storage format of the self and cross K/V rows (kv_dest())
   int kv_row = 256;               // bytes per K/V row of 64 elements
   // debug timeline (mt3_debug_trace_step): while `tracing` is set every decode GEMM / attention launch gets a slot
@@ -336,7 +338,8 @@ static unsigned long long* trace_slot(Model* m, const char* name) {
 // stays an encoder-only trade).  The non-cluster kernel (exact fp32) for K the cluster kernel does not tile.
 // name: the node's trace name (mt3_debug_trace_step).
 static int dec_gemm(Model* m, const char* name, const float* A, int lda, const float* W, int N, int K, int norm, int epi, float* C,
-                    int ldc, int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{}) {
+                    int ldc, int n_split, char* kv, const int* pos, cudaStream_t s, const KvStage& kst = KvStage{},
+                    const DecChain& ch = DecChain{}) {
   for (int r0 = 0; r0 < m->B; r0 += kDecBM) {
     DecGemmArgs a;
     memset(&a, 0, sizeof(a));
@@ -352,7 +355,7 @@ static int dec_gemm(Model* m, const char* name, const float* A, int lda, const f
     a.partial = m->dpartial;
     a.counters = m->dcounters;
     a.trace = trace_slot(m, name);
-    int rc = launch_dec_gemm_cluster(a, m->tc, s, r0 == 0 ? kst : KvStage{});
+    int rc = launch_dec_gemm_cluster(a, m->tc, s, r0 == 0 ? kst : KvStage{}, ch);
     if (rc == MT3_ERR_UNSUPPORTED) rc = launch_dec_gemm(a, s);
     MT3_TRY(rc);
   }
@@ -412,10 +415,26 @@ static KvStage kv_stage_for(const Model* m, int l, int len_add) {
   return k;
 }
 
-// fused RMSNorm + QKV projection + K/V cache append (layers.py:238-240, :272-289)
+// The programmatic edges of a decode GEMM node (DecChain): after_gemm -- its predecessor is a decode GEMM, which then lets
+// it launch early (the node loads its weights under it); late -- this node triggers its successor after the cluster
+// exchange.  Per edge, measured (DESIGN.md §3): MLP-in -> MLP-out and MLP-out -> QKV / logits trigger late; the cross
+// out-projection (1.2 MB of weights, 128 CTAs) triggers right after its wait, so that the MLP-in loads its weights under
+// it.  A GEMM before an attention kernel also triggers right after its wait: the attention kernel streams K/V under the
+// GEMM.  A GEMM after an attention kernel is launched plainly: started under the attention kernel it was slower (the
+// GEMM CTAs that find room start long before their cluster peers).  The argmax kernel -> next step's layer-0 QKV edge is
+// not taken: the first step of every graph has no kernel before its QKV, and at one edge per step it could save at most
+// about 1 us of a 580 us step.
+static DecChain dec_chain(const Model* m, bool after_gemm, bool late) {
+  DecChain c;
+  c.pdl = m->pdl_gemm && after_gemm;
+  c.late_trigger = m->pdl_gemm && late;
+  return c;
+}
+
+// fused RMSNorm + QKV projection + K/V cache append (layers.py:238-240, :272-289); layer l > 0 follows the MLP-out GEMM
 static int dec_layer_qkv(Model* m, const DecBranch& b, int l, cudaStream_t s) {
   return dec_gemm(m, "gemm_qkv_append", b.y, m->D, m->dec[l].wqkv, 3 * m->Q, m->D, 1, EPI_STORE, m->dq, m->Q, m->Q,
-                  kv_layer(m, m->skv, l, m->L), m->state, s);
+                  kv_layer(m, m->skv, l, m->L), m->state, s, KvStage{}, dec_chain(m, l > 0, false));
 }
 static int dec_layer_self(Model* m, int l, cudaStream_t s) {
   return dec_attention(m, m->dq, kv_layer(m, m->skv, l, m->L), m->L, m->state, 1, m->dao, s, nullptr, true);
@@ -442,10 +461,13 @@ static int dec_layer_cross(Model* m, const DecBranch& b, int l, cudaStream_t s) 
 static int dec_layer_mlp(Model* m, const DecBranch& b, int l, cudaStream_t s) {
   const DecLayer& w = m->dec[l];
   const int D = m->D, Q = m->Q, F = m->F;
-  MT3_TRY(dec_gemm(m, "gemm_attn_out", m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s));
-  MT3_TRY(dec_gemm(m, "gemm_mlp_in", b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, s));
+  MT3_TRY(dec_gemm(m, "gemm_attn_out", m->dao, Q, w.wo_c, D, Q, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s, KvStage{},
+                   dec_chain(m, false, false)));
+  MT3_TRY(dec_gemm(m, "gemm_mlp_in", b.y, D, w.wi, 2 * F, D, 1, EPI_GATED_GELU, m->dg, F, 2 * F, nullptr, nullptr, s, KvStage{},
+                   dec_chain(m, true, true)));
+  // followed by the next layer's QKV projection or by the logits projection
   MT3_TRY(dec_gemm(m, "gemm_mlp_out", m->dg, F, w.wo2, D, F, 0, EPI_RESIDUAL, b.y, D, D, nullptr, nullptr, s,
-                   l + 1 < m->Ld ? kv_stage_for(m, l + 1, 0) : KvStage{}));
+                   l + 1 < m->Ld ? kv_stage_for(m, l + 1, 0) : KvStage{}, dec_chain(m, true, true)));
   return MT3_OK;
 }
 
@@ -467,7 +489,7 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
     MT3_TRY(dec_layer_mlp(m, b, l, s));
   }
   MT3_TRY(dec_gemm(m, "gemm_logits", b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, s,
-                   kv_stage_for(m, 0, 1)));
+                   kv_stage_for(m, 0, 1), dec_chain(m, true, false)));
   float* y_next = loop_step ? m->dy : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L,
@@ -681,6 +703,8 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
     if (e_pfa) m->pf_attn = std::max(0, atoi(e_pfa));
     const char* e_pfk = getenv("MT3_PF_KV");
     if (e_pfk) m->pf_kv = std::max(0, atoi(e_pfk));
+    const char* e_pg = getenv("MT3_PDL_GEMM");
+    m->pdl_gemm = !(e_pg && e_pg[0] == '0');
   }
   m->kv_fmt = cfg->kv_cache_format;
   m->kv_row = kv_row_bytes(m->kv_fmt);

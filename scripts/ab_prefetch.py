@@ -5,7 +5,8 @@ encoder + cross-K/V + 1024 greedy steps, batch 64, L2 flushed between passes) an
 token streams bit for bit.
 
 The studies it was written for: L2 prefetch of the K/V tiles beyond the attention ring by the attention kernel itself
-(MT3_PF_ATTN); early L2 prefetch of each layer's first K/V tiles by the GEMM before its QKV projection (MT3_PF_KV).
+(MT3_PF_ATTN); early L2 prefetch of each layer's first K/V tiles by the GEMM before its QKV projection (MT3_PF_KV);
+programmatic edges between consecutive decode GEMM nodes (MT3_PDL_GEMM).
 
   python scripts/ab_prefetch.py [--kv p24] [--reps 3] [--settings "name:K=V,K=V;..."]
 """
@@ -18,7 +19,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-KNOBS = ("MT3_PF_ATTN", "MT3_PF_KV", "MT3_PDL")
+KNOBS = ("MT3_PF_ATTN", "MT3_PF_KV", "MT3_PDL", "MT3_PDL_GEMM")
 
 DEFAULT = ";".join(["off:MT3_PF_ATTN=0", "attn4:MT3_PF_ATTN=4", "attn8:MT3_PF_ATTN=8", "default:", "attn32:MT3_PF_ATTN=32",
                     "attn64:MT3_PF_ATTN=64", "off2:MT3_PF_ATTN=0"])

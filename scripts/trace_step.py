@@ -1,5 +1,9 @@
 """Device timeline of one greedy decode step (mt3_debug_trace_step): per graph node start / duration / gap to
-the previous node, and the internal phase split of CTA (0,0).  Run on a GPU box:  python scripts/trace_step.py"""
+the previous node, and the internal phase split of CTA (0,0).  Run on a GPU box:  python scripts/trace_step.py
+
+GEMM phases (us after CTA (0,0) started): PDL wait returned (a node launched under the GEMM before it starts early and waits
+there), weights landed and split into hi / lo tiles (tensor modes only, else 0), activations landed, multiply done,
+partials exchanged, reduce + epilogue issued.  Attention phases: first K tile landed, pass 1, softmax, pass 2, exit."""
 import ctypes as C
 import os
 import sys
@@ -11,6 +15,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mt3_b200 import _lib, inference  # noqa: E402
 
 SM_GHZ = 1.98      # H100 SXM maximum SM clock
+GEMM_WORDS = [6, 7, 2, 3, 4, 5]      # trace words of a GEMM slot in phase order (decode.cuh dec_cluster_body)
+ATTN_WORDS = [2, 3, 4, 5, 6, 7]      # attention slot; word 7 is unused
 
 
 def main():
@@ -33,14 +39,15 @@ def main():
         t = out[:n.value].astype(np.int64)
         t0 = t[0, 0]
         print(f"\n== decode step at cache position {pos}: {n.value} traced nodes (B={B})")
-        print(f"{'node':18s} {'start':>8s} {'dur':>7s} {'gap':>6s} | CTA(0,0) phases us: " "gemm: loads compute exchange reduce - | attn: first-K pass1 softmax pass2 exit")
+        print(f"{'node':18s} {'start':>8s} {'dur':>7s} {'gap':>6s} | CTA(0,0) phases us: "
+              "gemm: wait weights loads compute exchange reduce | attn: first-K pass1 softmax pass2 exit -")
         prev_end = t0
         agg = {}
         for i in range(n.value):
             st, en = t[i, 0], t[i, 1]
-            ph = t[i, 2:7] / (SM_GHZ * 1e3)
+            ph = t[i, GEMM_WORDS if nm[i].startswith('gemm') else ATTN_WORDS] / (SM_GHZ * 1e3)
             dur, gap = (en - st) / 1e3, (st - prev_end) / 1e3
-            a = agg.setdefault(nm[i], [0, 0.0, 0.0, np.zeros(5)])
+            a = agg.setdefault(nm[i], [0, 0.0, 0.0, np.zeros(6)])
             a[0] += 1; a[1] += dur; a[2] += gap; a[3] += ph
             if i < 8 and nm[i].startswith('gemm'):
                 print(f"{'':18s} SMs of tile 0's cluster (rank 0..7): " + ' '.join(str(int(x)) for x in t[i, 8:16]))
