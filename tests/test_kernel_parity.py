@@ -256,13 +256,15 @@ def _gemm_ref(A, W, rs, epi, R=None, pe=None, pe_T=None):
     return acc, cond
 
 
-def _run_gemm(kh, mode, M, N, K, epi, rs=False, pe_T=None, c_lo=False, inplace=False, seed=0, kv=None):
+def _run_gemm(kh, mode, M, N, K, epi, rs=False, pe_T=None, c_lo=False, inplace=False, seed=0, kv=None, AW=None):
     """One GEMM launch (mode "tf32" | "tf32x3" | "simt") into NaN-poisoned, padded buffers.  Returns (C [M, Nout] as
     float64 hi + lo, the C_hi / C_lo device buffers, ref, cond).  kv = (n_split, fmt, T, cap, H, C1 buffer) routes columns
-    >= n_split to the head-major K/V store."""
+    >= n_split to the head-major K/V store; AW = (A, W) replaces the random operands."""
     rng = np.random.default_rng(seed)
     A = _pos_mean(rng, (M, K))
     W = _pos_mean(rng, (K, N), 2.0 / K)
+    if AW is not None:
+        A, W = AW
     rsv = rng.uniform(0.5, 2.0, M).astype(np.float32) if rs else None
     Nout = N // 2 if epi == EPI_GATED_GELU else N
     n_split = kv[0] if kv else N
@@ -501,10 +503,15 @@ def test_enc_attention_tc(kh, T, B, H, sharp, split3, lo):
     the key-split form with KS = 2, 3, 4 (T = 512, 768, 1024) and its combine kernel, 2 .. 768 work items (below and far
     above the SM count: the persistent loop's barrier parity over many items per CTA), both precisions, out_lo null and
     not.  Measured worst err/bound: 3xTF32 0.21, TF32 0.18."""
-    Q = H * 64
     assert kh.kh_enc_attention_tc_supported(T), f"T={T} is documented as supported"
     rng = np.random.default_rng(T * 7 + B)
-    qkv = _attn_inputs(rng, B, T, H, sharp)
+    enc_attention_tc_check(kh, _attn_inputs(rng, B, T, H, sharp), B, T, H, split3, lo,
+                           f"tc attention T={T} B={B} H={H} sharp={sharp} split3={split3}")
+
+
+def enc_attention_tc_check(kh, qkv, B, T, H, split3, lo, name):
+    """enc_attention_tc_kernel on qkv [B*T, 3*H*64] against _attn_ref, per-element bars, NaN-poisoned outputs."""
+    Q = H * 64
     vt = _vt_host(qkv, B, T, H)
     o_ref, cond_p, cond_s = _attn_ref(qkv, B, T, H)
     if split3:
@@ -520,13 +527,13 @@ def test_enc_attention_tc(kh, T, B, H, sharp, split3, lo):
     if lo:
         got += ol[:B * T].double().cpu().numpy()
         assert (oh[:B * T].cpu().numpy().view(np.uint32) & 0x1FFF == 0).all()
-    _check(f"tc attention T={T} B={B} H={H} sharp={sharp} split3={split3}", got, o_ref, cond_p, TOL_ATT_PV[split3], cond_s,
-           TOL_ATT_S[split3])
+    worst = _check(name, got, o_ref, cond_p, TOL_ATT_PV[split3], cond_s, TOL_ATT_S[split3])
     w = np.zeros(oh.shape, bool)
     w[:B * T] = True
     _assert_poison("out_hi", oh, w)
     if lo:
         _assert_poison("out_lo", ol, w)
+    return worst
 
 
 @pytest.mark.parametrize("T", [1, 37, 100, 300, 768])
@@ -534,37 +541,45 @@ def test_enc_attention_fp32(kh, T):
     """enc_attention_kernel (exact fp32; every T, the path of T % 8 != 0 and of T > 256 that is not a multiple of 256).
     Measured worst err/bound: 0.22."""
     B, H = 2, 2
-    Q = H * 64
     rng = np.random.default_rng(T)
-    qkv = _attn_inputs(rng, B, T, H, sharp=T % 2 == 0)
+    enc_attention_fp32_check(kh, _attn_inputs(rng, B, T, H, sharp=T % 2 == 0), B, T, H, f"fp32 attention T={T}")
+
+
+def enc_attention_fp32_check(kh, qkv, B, T, H, name):
+    """enc_attention_kernel on qkv [B*T, 3*H*64] (rows past B*T NaN), with and without out_lo, against _attn_ref."""
+    Q = H * 64
     o_ref, cond_p, cond_s = _attn_ref(qkv, B, T, H)
     buf = _nan(B * T + 8, 3 * Q)                               # rows past B*T: NaN the kernel must not read
     buf[:B * T] = _dev(qkv)
+    worst = 0.0
     for lo in (False, True):
         oh, ol = _nan(B * T + 5, Q), (_nan(B * T + 5, Q) if lo else None)
         _call(kh, "kh_enc_attention_fp32", _p(buf), B, T, H, _p(oh), _p(ol))
         got = oh[:B * T].double().cpu().numpy() + (ol[:B * T].double().cpu().numpy() if lo else 0)
-        _check(f"fp32 attention T={T} lo={lo}", got, o_ref, cond_p, TOL_ENC_ATT_P, cond_s, TOL_ENC_ATT_S)
+        worst = max(worst, _check(f"{name} lo={lo}", got, o_ref, cond_p, TOL_ENC_ATT_P, cond_s, TOL_ENC_ATT_S))
         w = np.zeros(oh.shape, bool)
         w[:B * T] = True
         _assert_poison("out", oh, w)
+    return worst
 
 
 # ------------------------------------------------------------------------------------------------
 # decode GEMMs: sgemm_dec_cluster_kernel, sgemm_dec_kernel, sgemm_dec_cluster2_kernel
 # ------------------------------------------------------------------------------------------------
-def _dec_setup(M, N, K, epi, norm, seed):
+def _dec_setup(M, N, K, epi, norm, seed, AW=None):
     rng = np.random.default_rng(seed)
     A = _pos_mean(rng, (M, K), 2.0)
     W = _pos_mean(rng, (K, N), 2.0 / K)
+    if AW is not None:
+        A, W = AW
     R = _pos_mean(rng, (M, N)) if epi == EPI_RESIDUAL else None
     rs = 1.0 / np.sqrt((A.astype(np.float64) ** 2).mean(1) + 1e-6) if norm else None
     ref, cond = _gemm_ref(A, W, rs, epi, R)
     return A, W, R, ref, cond
 
 
-def _dec_run(kh, kernel, M, N, K, epi, norm, inplace, seed, kv=None, ssq=False):
-    A, W, R, ref, cond = _dec_setup(M, N, K, epi, norm, seed)
+def _dec_run(kh, kernel, M, N, K, epi, norm, inplace, seed, kv=None, ssq=False, AW=None):
+    A, W, R, ref, cond = _dec_setup(M, N, K, epi, norm, seed, AW)
     Nout = N // 2 if epi == EPI_GATED_GELU else N
     n_split = kv[0] if kv else N
     ncols = min(Nout, n_split)
@@ -704,18 +719,26 @@ def test_dec_attention(kh, fmt, L, B, H, pf, ssq, len_ptr):
     be read.  The reference is float64 over the DECODED stored rows, so every format meets the fp32 bar (the formats'
     own rounding is the codec test's).  len = *len_ptr + len_add, q scaled by rsqrt(sum q_ssq / q_dim + eps).
     Measured worst err/bound: 0.10."""
-    cap, ldq, q_off, ldo = L + 9, H * 64 + 8, 4, H * 64 + 4
+    H_ldq = H * 64 + 8
     rng = np.random.default_rng(L * 3 + fmt)
     rows = rng.standard_normal((B, 2, H, L, 64)).astype(np.float32) * np.float32(0.4)
     rows[:, 1] = rng.uniform(-0.5, 1.0, (B, H, L, 64))
+    q = _pos_mean(rng, (B, H_ldq), 1.0)
+    part = rng.uniform(100.0, 200.0, (B, 17)).astype(np.float32)
+    dec_attention_check(kh, fmt, rows, q, part if ssq else None, pf, len_ptr, f"decode attention fmt={fmt} L={L} B={B}")
+
+
+def dec_attention_check(kh, fmt, rows, q, part, pf, len_ptr, name, q_off=4, qd=512.0, eps=1e-6):
+    """dec_attention_bulk_kernel<fmt> on K/V rows [B, 2, H, L, 64] (fp32 values, stored in format fmt; rows past L inside
+    cap NaN) and queries q [B, ldq] (head h at columns q_off + 64 h), scaled by rsqrt(sum part[:, :-1] / qd + eps) when
+    part [B, n + 1] is given, against float64 over the DECODED stored rows."""
+    B, _, H, L, _ = rows.shape
+    cap, ldq, ldo = L + 9, q.shape[1], H * 64 + 4
     kvb = np.full((B, 2, H, cap, ROWB[fmt]), 255, np.uint8)
     kvb[:, :, :, :L] = encode_rows(rows, fmt)
     kv_vals = decode_rows(kvb[:, :, :, :L], fmt)                   # what is stored
-    q = _pos_mean(rng, (B, ldq), 1.0)
-    n_ssq = 16
-    part = rng.uniform(100.0, 200.0, (B, n_ssq + 1)).astype(np.float32)
-    qd, eps = 512.0, 1e-6
-    rs = 1.0 / np.sqrt(part[:, :n_ssq].astype(np.float64).sum(1) / qd + eps) if ssq else np.ones(B)
+    n_ssq = 0 if part is None else part.shape[1] - 1
+    rs = np.ones(B) if part is None else 1.0 / np.sqrt(part[:, :n_ssq].astype(np.float64).sum(1) / qd + eps)
     qh = q[:, q_off:q_off + H * 64].astype(np.float64).reshape(B, H, 64) * rs[:, None, None]
     k, v = kv_vals[:, 0], kv_vals[:, 1]
     S = np.einsum("bhd,bhkd->bhk", qh, k)
@@ -726,17 +749,18 @@ def test_dec_attention(kh, fmt, L, B, H, pf, ssq, len_ptr):
     pA = p * np.einsum("bhd,bhkd->bhk", np.abs(qh), np.abs(k))
     cond_s = np.einsum("bhk,bhkd->bhd", pA, np.abs(v)) + np.abs(o) * pA.sum(-1, keepdims=True)
     d_kv = _dev(kvb.reshape(-1))
-    d_q, d_ssq = _dev(q), _dev(part)
+    d_q, d_ssq = _dev(q), (_dev(part) if part is not None else None)
     lenp = torch.tensor([L - 1], dtype=torch.int32, device=DEV) if len_ptr else None
     out = _nan(B + 1, ldo)
     _call(kh, "kh_dec_attention", fmt, _p(d_q), ldq, q_off, _p(d_kv), H, cap, _p(lenp), 1 if len_ptr else L, L, _p(out), ldo,
-          _p(d_ssq) if ssq else None, n_ssq, n_ssq + 1, qd, eps, pf, B)
+          _p(d_ssq), n_ssq, n_ssq + 1, qd, eps, pf, B)
     got = out[:B, :H * 64].double().cpu().numpy()
-    _check(f"decode attention fmt={fmt} L={L} B={B}", got, o.reshape(B, H * 64), cond_p.reshape(B, H * 64), TOL_DEC_ATT_P,
-           cond_s.reshape(B, H * 64), TOL_DEC_ATT_S)
+    worst = _check(name, got, o.reshape(B, H * 64), cond_p.reshape(B, H * 64), TOL_DEC_ATT_P, cond_s.reshape(B, H * 64),
+                   TOL_DEC_ATT_S)
     w = np.zeros(out.shape, bool)
     w[:B, :H * 64] = True
     _assert_poison("out", out, w)
+    return S, worst
 
 
 # ------------------------------------------------------------------------------------------------
