@@ -181,6 +181,29 @@ enum {
 int mt3_generate(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                  int32_t* steps_run, void* stream);
 
+/* Transformer.decode(decode=False) / Transformer.__call__ (network.py:303-409 with decode=False, :196-262) and the token
+ * scores of T5X's EncoderDecoderModel.score_batch (z_loss = 0): the teacher-forced decoder pass over all L positions at
+ * once, from the caller's `encoded` DEV f32 [B, T, emb_dim] (the output of mt3_encode).
+ *   decoder_input_tokens, decoder_target_tokens DEV i32 [B, L]; loss_weights DEV i32 [B, L] or NULL (= target > 0).
+ *   Self-attention mask make_decoder_mask(decoder_target_tokens): query i sees key j iff j <= i and target[j] > 0;
+ *   positions are arange(L); cross-attention sees all T encoder positions.
+ *   logits DEV f32 [B, L, vocab] (16-byte aligned) or NULL; token_scores DEV f32 [B, L] or NULL:
+ *   (logits[b, i, target] - logsumexp(logits[b, i, :])) * weight[b, i].  Not both NULL.
+ *   Positions with target == 0 (padding) get the causal, key-masked result -- finite, 0 where no key is visible -- not the
+ *   reference's all-masked row (DESIGN.md section 1), and score 0 under the default weights.
+ * All K/V of the pass are float32 whatever kv_cache_format is, and live in `workspace` DEV (256-byte aligned,
+ * mt3_teacher_forced_workspace_bytes); the decode state (workspace of mt3_model_set_workspace, K/V caches, position,
+ * captured graphs) is not touched.  In the wgmma gemm modes the first call builds K-major copies of the decoder weights
+ * (TF32X3 ~183 MB, TF32 ~92 MB at the mt3 shapes), owned by the model and freed by mt3_model_destroy.
+ * Every argument is checked before any CUDA call: MT3_ERR_BAD_ARG (null handle / input, both outputs NULL),
+ * MT3_ERR_SHAPE (batch, input_length or target_length outside (0, the model's limit]), MT3_ERR_WORKSPACE (short or
+ * misaligned workspace). */
+int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* m, int32_t batch, int32_t input_length, int32_t target_length);
+int mt3_decode_teacher_forced(mt3_model* m, const float* encoded, int32_t batch, int32_t input_length,
+                              const int32_t* decoder_input_tokens, const int32_t* decoder_target_tokens,
+                              const int32_t* loss_weights, int32_t target_length, float* logits, float* token_scores,
+                              void* workspace, int64_t workspace_bytes, void* stream);
+
 /* GenericTokenVocabulary._decode_tf (vocabularies.py:241-271): ids DEV i32 [B, L]
  * -> out DEV i32 [B, L] with id-3, EOS-and-after = -1, invalid = -2. */
 int mt3_vocab_decode(const int32_t* ids, int32_t batch, int32_t length, int32_t num_regular_tokens, int32_t* out,

@@ -25,6 +25,7 @@ EXPORTS = [
     "mt3_model_num_params", "mt3_model_param_offset", "mt3_model_create", "mt3_model_destroy",
     "mt3_workspace_bytes", "mt3_model_set_workspace", "mt3_encode", "mt3_cross_kv", "mt3_decode_step",
     "mt3_generate", "mt3_vocab_decode", "mt3_dot_product_attention_f32", "mt3_debug_launch", "mt3_debug_trace_step",
+    "mt3_teacher_forced_workspace_bytes", "mt3_decode_teacher_forced",
 ]
 
 
@@ -84,6 +85,9 @@ def load() -> C.CDLL:
     lib.mt3_vocab_decode.argtypes = [i32p, i32, i32, i32, i32p, vp]
     lib.mt3_dot_product_attention_f32.argtypes = [f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p, vp]
     lib.mt3_debug_launch.argtypes = [vp, i32, i32, i32, vp]
+    lib.mt3_teacher_forced_workspace_bytes.argtypes = [vp, i32, i32, i32]
+    lib.mt3_teacher_forced_workspace_bytes.restype = i64
+    lib.mt3_decode_teacher_forced.argtypes = [vp, f32p, i32, i32, i32p, i32p, i32p, i32, f32p, f32p, vp, i64, vp]
     lib.mt3_debug_trace_step.argtypes = [vp, i32, vp, i32, C.c_char_p, i32, C.POINTER(C.c_int32), vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here = header/library mismatch

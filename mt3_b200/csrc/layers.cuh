@@ -85,34 +85,41 @@ inline int launch_rmsnorm(const float* x, const float* x_lo, int ldx, int M, int
 // ---------------------------------------------------------------------------------
 constexpr int kHD = 64;   // head_dim the kernels are specialised for (gin/model.gin:54)
 
-__global__ void __launch_bounds__(256)
-enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float* __restrict__ out,
-                     float* __restrict__ out_lo, int ldo) {
+// The work of one CTA, shared by the encoder kernel and the decoder's teacher-forced forms: queries of head h at columns
+// q_col0 + 64 h of q's rows [b Tq, (b + 1) Tq) (row pitch ldq), keys / values at k_col0 / v_col0 + 64 h of kv's rows
+// [b Tk, (b + 1) Tk) (row pitch ldkv).  CAUSAL: query i sees key j iff j <= i, j < n_valid and key_valid[b * n_valid + j]
+// > 0; key tiles past the CTA's last query are not read, and a row with no visible key writes 0.
+template <bool CAUSAL>
+__device__ __forceinline__ void attention_fp32_body(const float* __restrict__ q, int ldq, int q_col0, const float* __restrict__ kv, int ldkv,
+                                                    int k_col0, int v_col0, int Tq, int Tk, int H, float* __restrict__ out,
+                                                    float* __restrict__ out_lo, int ldo, const int* __restrict__ key_valid, int n_valid) {
   extern __shared__ __align__(16) float sm[];
   constexpr int QT = 32, KT = 64;
-  const int SP = T + 4;
+  const int SP = Tk + 4;
   float* sQ = sm;                 // [QT][64]
-  float* sS = sQ + QT * kHD;      // [QT][T+4]
+  float* sS = sQ + QT * kHD;      // [QT][Tk+4]
   float* sT = sS + QT * SP;       // [64][KT+4]  K tile transposed ([d][k]) / V tile [k][d+4]
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * QT;
   const int tid = threadIdx.x;
-  const int qoff = h * kHD, koff = H * kHD + h * kHD, voff = 2 * H * kHD + h * kHD;
-  const float* base = qkv + (long long)b * T * ld;
+  const int qoff = q_col0 + h * kHD, koff = k_col0 + h * kHD, voff = v_col0 + h * kHD;
+  const float* qbase = q + (long long)b * Tq * ldq;
+  const float* base = kv + (long long)b * Tk * ldkv;
+  const int kend = CAUSAL ? min(Tk, q0 + QT) : Tk;      // keys any row of this CTA can see lie below kend
 
   for (int i = tid; i < QT * kHD / 4; i += 256) {
     const int r = i / (kHD / 4), c4 = i % (kHD / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (q0 + r < T) v = *reinterpret_cast<const float4*>(base + (long long)(q0 + r) * ld + qoff + c4 * 4);
+    if (q0 + r < Tq) v = *reinterpret_cast<const float4*>(qbase + (long long)(q0 + r) * ldq + qoff + c4 * 4);
     *reinterpret_cast<float4*>(sQ + r * kHD + c4 * 4) = v;
   }
   // S = Q K^T : thread -> 2 query rows x 4 keys
   const int tq = tid / 16, tk = tid % 16;     // tq in [0,16): rows tq, tq+16 ; tk: keys tk*4..+3
-  for (int k0 = 0; k0 < T; k0 += KT) {
+  for (int k0 = 0; k0 < kend; k0 += KT) {
     __syncthreads();
     for (int i = tid; i < KT * kHD / 4; i += 256) {
       const int r = i / (kHD / 4), c4 = i % (kHD / 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (k0 + r < T) v = *reinterpret_cast<const float4*>(base + (long long)(k0 + r) * ld + koff + c4 * 4);
+      if (k0 + r < kend) v = *reinterpret_cast<const float4*>(base + (long long)(k0 + r) * ldkv + koff + c4 * 4);
       sT[(c4 * 4 + 0) * (KT + 4) + r] = v.x;
       sT[(c4 * 4 + 1) * (KT + 4) + r] = v.y;
       sT[(c4 * 4 + 2) * (KT + 4) + r] = v.z;
@@ -123,18 +130,24 @@ enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float*
 #pragma unroll 8
     for (int d = 0; d < kHD; ++d) {
       const float q_0 = sQ[tq * kHD + d], q_1 = sQ[(tq + 16) * kHD + d];
-      const float4 kv = *reinterpret_cast<const float4*>(sT + d * (KT + 4) + tk * 4);
-      a0[0] = fmaf(q_0, kv.x, a0[0]); a0[1] = fmaf(q_0, kv.y, a0[1]);
-      a0[2] = fmaf(q_0, kv.z, a0[2]); a0[3] = fmaf(q_0, kv.w, a0[3]);
-      a1[0] = fmaf(q_1, kv.x, a1[0]); a1[1] = fmaf(q_1, kv.y, a1[1]);
-      a1[2] = fmaf(q_1, kv.z, a1[2]); a1[3] = fmaf(q_1, kv.w, a1[3]);
+      const float4 kv4 = *reinterpret_cast<const float4*>(sT + d * (KT + 4) + tk * 4);
+      a0[0] = fmaf(q_0, kv4.x, a0[0]); a0[1] = fmaf(q_0, kv4.y, a0[1]);
+      a0[2] = fmaf(q_0, kv4.z, a0[2]); a0[3] = fmaf(q_0, kv4.w, a0[3]);
+      a1[0] = fmaf(q_1, kv4.x, a1[0]); a1[1] = fmaf(q_1, kv4.y, a1[1]);
+      a1[2] = fmaf(q_1, kv4.z, a1[2]); a1[3] = fmaf(q_1, kv4.w, a1[3]);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int k = k0 + tk * 4 + j;
-      if (k < T) {
-        sS[tq * SP + k] = a0[j];
-        sS[(tq + 16) * SP + k] = a1[j];
+      if (k < kend) {
+        if (CAUSAL) {
+          const bool ok = k < n_valid && key_valid[(long long)b * n_valid + k] > 0;
+          sS[tq * SP + k] = (ok && k <= q0 + tq) ? a0[j] : -INFINITY;
+          sS[(tq + 16) * SP + k] = (ok && k <= q0 + tq + 16) ? a1[j] : -INFINITY;
+        } else {
+          sS[tq * SP + k] = a0[j];
+          sS[(tq + 16) * SP + k] = a1[j];
+        }
       }
     }
   }
@@ -145,32 +158,33 @@ enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float*
     for (int r = warp * 4; r < warp * 4 + 4; ++r) {
       float* row = sS + r * SP;
       float mx = -INFINITY;
-      for (int k = lane; k < T; k += 32) mx = fmaxf(mx, row[k]);
+      for (int k = lane; k < kend; k += 32) mx = fmaxf(mx, row[k]);
       mx = warp_max(mx);
+      if (CAUSAL && mx == -INFINITY) mx = 0.f;         // no visible key: every weight is exp(-inf) = 0
       float sum = 0.f;
-      for (int k = lane; k < T; k += 32) {
+      for (int k = lane; k < kend; k += 32) {
         const float e = expf(row[k] - mx);
         row[k] = e;
         sum += e;
       }
       sum = warp_sum(sum);
-      const float inv = 1.0f / sum;
-      for (int k = lane; k < T; k += 32) row[k] *= inv;
+      const float inv = (CAUSAL && !(sum > 0.f)) ? 0.f : 1.0f / sum;
+      for (int k = lane; k < kend; k += 32) row[k] *= inv;
     }
   }
   // O = P V : thread -> 2 query rows x 4 dims
   float o0[4] = {0.f, 0.f, 0.f, 0.f}, o1[4] = {0.f, 0.f, 0.f, 0.f};
   const int td = tid % 16;   // dims td*4..+3
-  for (int k0 = 0; k0 < T; k0 += KT) {
+  for (int k0 = 0; k0 < kend; k0 += KT) {
     __syncthreads();
     for (int i = tid; i < KT * kHD / 4; i += 256) {
       const int r = i / (kHD / 4), c4 = i % (kHD / 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (k0 + r < T) v = *reinterpret_cast<const float4*>(base + (long long)(k0 + r) * ld + voff + c4 * 4);
+      if (k0 + r < kend) v = *reinterpret_cast<const float4*>(base + (long long)(k0 + r) * ldkv + voff + c4 * 4);
       *reinterpret_cast<float4*>(sT + r * (kHD + 4) + c4 * 4) = v;
     }
     __syncthreads();
-    const int kmax = min(KT, T - k0);
+    const int kmax = min(KT, kend - k0);
     for (int k = 0; k < kmax; ++k) {
       const float p0 = sS[tq * SP + k0 + k], p1 = sS[(tq + 16) * SP + k0 + k];
       const float4 vv = *reinterpret_cast<const float4*>(sT + k * (kHD + 4) + td * 4);
@@ -180,9 +194,9 @@ enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float*
       o1[2] = fmaf(p1, vv.z, o1[2]); o1[3] = fmaf(p1, vv.w, o1[3]);
     }
   }
-  const long long obase = (long long)b * T * ldo + h * kHD + td * 4;
+  const long long obase = (long long)b * Tq * ldo + h * kHD + td * 4;
   auto store = [&](int row, const float (&o)[4]) {
-    if (row >= T) return;
+    if (row >= Tq) return;
     const long long off = obase + (long long)row * ldo;
     if (out_lo) {
       float hi[4], lo[4];
@@ -198,6 +212,20 @@ enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float*
   store(q0 + tq + 16, o1);
 }
 
+__global__ void __launch_bounds__(256)
+enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float* __restrict__ out,
+                     float* __restrict__ out_lo, int ldo) {
+  attention_fp32_body<false>(qkv, ld, 0, qkv, ld, H * kHD, 2 * H * kHD, T, T, H, out, out_lo, ldo, nullptr, 0);
+}
+
+template <bool CAUSAL>
+__global__ void __launch_bounds__(256)
+attention_fp32_kernel(const float* __restrict__ q, int ldq, int q_col0, const float* __restrict__ kv, int ldkv, int k_col0, int v_col0,
+                      int Tq, int Tk, int H, float* __restrict__ out, float* __restrict__ out_lo, int ldo,
+                      const int* __restrict__ key_valid, int n_valid) {
+  attention_fp32_body<CAUSAL>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, key_valid, n_valid);
+}
+
 // sQ, sS and sT of enc_attention_kernel; the scores of all T keys bound T.
 constexpr size_t kEncAttMaxSmem = 200 * 1024;
 inline size_t enc_attention_smem(int T) { return (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float); }
@@ -211,6 +239,27 @@ inline int launch_enc_attention(const float* qkv, int ld, int T, int H, int B, f
     attr_done = true;
   }
   enc_attention_kernel<<<dim3(cdiv(T, 32), H, B), 256, smem, s>>>(qkv, ld, T, H, out, out_lo, ldo);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// The decoder's teacher-forced forms (attention_fp32_body): causal self-attention over the [B*Tq, 3Q] qkv rows with per-key
+// validity (key_valid != null), or cross-attention of q [B*Tq, ldq] over kv [B*Tk, ldkv].  out [B*Tq, H*64].
+inline int launch_attention_fp32(const float* q, int ldq, int q_col0, const float* kv, int ldkv, int k_col0, int v_col0, int Tq, int Tk, int H,
+                                 int B, float* out, float* out_lo, int ldo, const int* key_valid, int n_valid, cudaStream_t s) {
+  const size_t smem = enc_attention_smem(Tk);
+  MT3_REQUIRE(smem <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "fp32 attention: Tk=%d too long", Tk);
+  static bool attr_done = false;
+  if (!attr_done) {
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
+    attr_done = true;
+  }
+  const dim3 grid(cdiv(Tq, 32), H, B);
+  if (key_valid)
+    attention_fp32_kernel<true><<<grid, 256, smem, s>>>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, key_valid, n_valid);
+  else
+    attention_fp32_kernel<false><<<grid, 256, smem, s>>>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, nullptr, 0);
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -606,6 +655,101 @@ __global__ void transpose_split_kernel(const float* __restrict__ src, int K, int
       }
     }
   }
+}
+
+// ---------------------------------------------------------------------------------
+// Teacher-forced decoder input: y[b * Lp + i, :] = E[tok[b, i], :] + PE[i, :] for i < L (network.py:211-217; positions
+// are arange(L)), 0 for the padding rows L <= i < Lp.  Ids outside [0, vocab) are clamped as in embed_kernel.
+// y_lo != null: the row is written as a tf32 hi/lo pair.  One CTA per row.
+// ---------------------------------------------------------------------------------
+__global__ void embed_seq_kernel(const int* __restrict__ tok, int L, int Lp, const float* __restrict__ emb, int D, int vocab,
+                                 const float* __restrict__ pe, float* __restrict__ y, float* __restrict__ y_lo) {
+  const int row = blockIdx.x, b = row / Lp, i = row % Lp;
+  float4* o = reinterpret_cast<float4*>(y + (long long)row * D);
+  float4* ol = y_lo ? reinterpret_cast<float4*>(y_lo + (long long)row * D) : nullptr;
+  if (i >= L) {
+    for (int c = threadIdx.x; c < D / 4; c += blockDim.x) {
+      o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (ol) ol[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    return;
+  }
+  const int t = min(max(tok[(long long)b * L + i], 0), vocab - 1);
+  const float4* e = reinterpret_cast<const float4*>(emb + (long long)t * D);
+  const float4* p = reinterpret_cast<const float4*>(pe + (long long)i * D);
+  for (int c = threadIdx.x; c < D / 4; c += blockDim.x) {
+    const float4 a = __ldg(e + c), q = __ldg(p + c);
+    const float4 v = make_float4(a.x + q.x, a.y + q.y, a.z + q.z, a.w + q.w);
+    if (ol) {
+      float4 h, l;
+      split_tf32(v.x, h.x, l.x); split_tf32(v.y, h.y, l.y); split_tf32(v.z, h.z, l.z); split_tf32(v.w, h.w, l.w);
+      o[c] = h;
+      ol[c] = l;
+    } else {
+      o[c] = v;
+    }
+  }
+}
+
+inline int launch_embed_seq(const int* tok, int B, int L, int Lp, const float* emb, int D, int vocab, const float* pe, float* y, float* y_lo,
+                            cudaStream_t s) {
+  embed_seq_kernel<<<B * Lp, 128, 0, s>>>(tok, L, Lp, emb, D, vocab, pe, y, y_lo);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// ---------------------------------------------------------------------------------
+// Token score of T5X score_batch (z_loss = 0): score[b, i] = (x[t] - logsumexp(x)) * w over the logits row x of position
+// (b, i), t = target[b, i] (clamped into [0, V)), w = weight[b, i] or, without weights, target > 0; a weight of 0 scores
+// exactly 0.  One CTA per row of a chunk of padded rows: logits [n, V] hold rows row0 .. row0 + n - 1 of [B * Lp]; rows
+// with i >= L are padding and skipped.  logits_out [B, L, V] (optional) receives a copy of each row.
+// ---------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+token_score_kernel(const float* __restrict__ logits, int V, int row0, int Lp, int L, const int* __restrict__ target,
+                   const int* __restrict__ weight, float* __restrict__ scores, float* __restrict__ logits_out) {
+  __shared__ float red[8];
+  const int g = row0 + blockIdx.x;
+  const int b = g / Lp, i = g % Lp;
+  if (i >= L) return;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* x = logits + (long long)blockIdx.x * V;
+  const long long pos = (long long)b * L + i;
+  if (logits_out) {
+    const float4* src = reinterpret_cast<const float4*>(x);
+    float4* dst = reinterpret_cast<float4*>(logits_out + pos * V);
+    for (int c = tid; c < V / 4; c += 256) dst[c] = src[c];
+  }
+  if (!scores) return;
+  float mx = -INFINITY;
+  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
+  mx = warp_max(mx);
+  if (lane == 0) red[warp] = mx;
+  __syncthreads();
+  mx = red[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
+  __syncthreads();
+  float se = 0.f;
+  for (int c = tid; c < V; c += 256) se += expf(x[c] - mx);
+  se = warp_sum(se);
+  if (lane == 0) red[warp] = se;
+  __syncthreads();
+  if (tid == 0) {
+    float tot = 0.f;
+    for (int w = 0; w < 8; ++w) tot += red[w];
+    const int tg = target[pos];
+    const float wt = weight ? (float)weight[pos] : (tg > 0 ? 1.f : 0.f);
+    const int t = min(max(tg, 0), V - 1);
+    scores[pos] = wt != 0.f ? (x[t] - (mx + logf(tot))) * wt : 0.f;
+  }
+}
+
+inline int launch_token_score(const float* logits, int V, int row0, int n_rows, int Lp, int L, const int* target, const int* weight,
+                              float* scores, float* logits_out, cudaStream_t s) {
+  if (n_rows <= 0) return MT3_OK;
+  token_score_kernel<<<n_rows, 256, 0, s>>>(logits, V, row0, Lp, L, target, weight, scores, logits_out);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
 }
 
 }  // namespace mt3

@@ -78,7 +78,10 @@ struct TcW { float* hi = nullptr; float* lo = nullptr; TcOperand op; int K = 0, 
 struct Act { float* hi = nullptr; float* lo = nullptr; TcOperand op; };
 
 struct EncLayer { float *wqkv, *wo, *wi, *wo2; TcW t_wqkv, t_wo, t_wi, t_wo2; };
-struct DecLayer { float *wqkv, *wo, *wq_c, *wkv_c, *wo_c, *wi, *wo2; float* wc1 = nullptr; TcW t_wkv_c; };   // wc1: [Q+D, Q] = [Wo.Wq ; Wq]
+struct DecLayer {
+  float *wqkv, *wo, *wq_c, *wkv_c, *wo_c, *wi, *wo2; float* wc1 = nullptr; TcW t_wkv_c;   // wc1: [Q+D, Q] = [Wo.Wq ; Wq]
+  TcW t_wqkv, t_wo, t_wq_c, t_wo_c, t_wi, t_wo2;   // teacher-forced pass only: built on its first call (ensure_tf_weights)
+};
 
 struct Model {
   mt3_model_config cfg;
@@ -112,6 +115,8 @@ struct Model {
   float* emb = nullptr;
   std::vector<DecLayer> dec;
   float* w_logits = nullptr;
+  TcW t_w_logits;                 // teacher-forced pass only, like DecLayer::t_wqkv ...
+  float* slab_tf = nullptr;       // K-major (and hi/lo) decoder weights of the teacher-forced pass; null until its first call
   float* pe = nullptr;            // [pe_rows, D] sinusoid table (FixedEmbed.max_length, layers.py:565)
   int pe_rows = 2048;
 
@@ -558,6 +563,185 @@ static int ensure_graph(Model* m, int mode, int nsteps = 1) {
   return MT3_OK;
 }
 
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Teacher-forced decoder pass (network.py:196-262, :327-335 with decode=False): all L positions at once, M = B * Lp rows
+// (Lp = L rounded up to the attention query tile; rows past L are zero inputs that causality keeps away from the real
+// positions).  The encoder's GEMM epilogues and back ends; causal self-attention and cross-attention on the wgmma kernel
+// (attention_tc.cuh) or exactly in fp32 (layers.cuh); K/V in float32 that live in the caller's workspace for the pass
+// only.  Touches none of the decode state (model workspace, caches, position, graphs).
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kTfLogitRows = 8192;   // logits rows per chunk of the logits GEMM + score kernel (50 MB at V = 1536)
+
+static int tf_pad(int L) { return cdiv(L, kAtQ) * kAtQ; }
+static bool tf_self_tc(const Model* m) { return m->tc && m->tc_attn_ok; }
+static bool tf_cross_tc(const Model* m, int T) { return m->tc && m->tc_attn_ok && enc_attention_tc_supported(T); }
+
+struct TfLayout {
+  int64_t y, y_lo, rstd, qkv, qkv_lo, vt, vt_lo, ao, ao_lo, qc, qc_lo, enc, enc_lo, ckv, ckv_lo, cvt, cvt_lo, g, g_lo, scratch, logits, total;
+};
+static TfLayout tf_layout(const Model* m, int B, int T, int L) {
+  TfLayout w;
+  int64_t off = 0;
+  auto take = [&](int64_t bytes) { int64_t r = off; off += align_up(bytes, 256); return r; };
+  const int Lp = tf_pad(L);
+  const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T, D = m->D, Q = m->Q, F = m->F, V = m->V;
+  const bool s3 = m->split3, tcs = tf_self_tc(m), tcc = tf_cross_tc(m, T);
+  w.y = take(M * D * 4);                          // residual stream (hi/lo in TF32X3)
+  w.y_lo = take(s3 ? M * D * 4 : 0);
+  w.rstd = take(M * 4);
+  w.qkv = take(M * 3 * Q * 4);
+  w.qkv_lo = take(s3 && tcs ? M * 3 * Q * 4 : 0);
+  w.vt = take(tcs ? M * Q * 4 : 0);               // per-head V^T [B*H*64, Lp] of the wgmma self-attention
+  w.vt_lo = take(s3 && tcs ? M * Q * 4 : 0);
+  w.ao = take(M * Q * 4);                         // attention output (self, then cross)
+  w.ao_lo = take(s3 ? M * Q * 4 : 0);
+  w.qc = take(M * Q * 4);                         // cross-attention queries
+  w.qc_lo = take(s3 && tcc ? M * Q * 4 : 0);
+  w.enc = take(s3 ? Me * D * 4 : 0);              // tf32 hi/lo split of `encoded` (TF32X3)
+  w.enc_lo = take(s3 ? Me * D * 4 : 0);
+  w.ckv = take(Me * 2 * Q * 4);                   // one layer's cross K | V [B*T, 2Q] (V as V^T in cvt on the wgmma path)
+  w.ckv_lo = take(s3 && tcc ? Me * 2 * Q * 4 : 0);
+  w.cvt = take(tcc ? Me * Q * 4 : 0);
+  w.cvt_lo = take(s3 && tcc ? Me * Q * 4 : 0);
+  w.g = take(M * F * 4);
+  w.g_lo = take(s3 ? M * F * 4 : 0);
+  w.scratch = take(std::max(tcs ? attention_tc_scratch_floats(B, Lp, Lp, m->H, true) : 0,
+                            tcc ? attention_tc_scratch_floats(B, Lp, T, m->H, false) : 0) * 4);
+  w.logits = take(std::min(M, (int64_t)kTfLogitRows) * V * 4);
+  w.total = off;
+  return w;
+}
+
+static int64_t tf_weight_floats(const Model* m) {
+  const int64_t D = m->D, Q = m->Q, F = m->F, V = m->V;
+  const int64_t per_layer = D * 3 * Q + Q * D + D * Q + Q * D + D * 2 * F + F * D;
+  return (m->Ld * per_layer + D * V) * (m->split3 ? 2 : 1);
+}
+
+// K-major (hi/lo in TF32X3) copies of the decoder weights the pass multiplies on the wgmma path: made on its first call,
+// so that a model that only transcribes keeps its footprint (TF32X3 ~183 MB, TF32 ~92 MB at the mt3 shapes).
+static int ensure_tf_weights(Model* m, cudaStream_t s) {
+  if (!m->tc || m->slab_tf) return MT3_OK;
+  float* slab = nullptr;
+  MT3_CUDA_CHECK(cudaMalloc((void**)&slab, (size_t)tf_weight_floats(m) * sizeof(float)));
+  float* cur = slab;
+  const int D = m->D, Q = m->Q, F = m->F;
+  int rc = MT3_OK;
+  for (int l = 0; l < m->Ld && rc == MT3_OK; ++l) {
+    DecLayer& L = m->dec[l];
+    rc = prep_tc_weight(m, s, L.wqkv, D, 3 * Q, cur, &L.t_wqkv);
+    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo, Q, D, cur, &L.t_wo);
+    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wq_c, D, Q, cur, &L.t_wq_c);
+    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo_c, Q, D, cur, &L.t_wo_c);
+    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wi, D, 2 * F, cur, &L.t_wi);
+    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo2, F, D, cur, &L.t_wo2);
+  }
+  if (rc == MT3_OK) rc = prep_tc_weight(m, s, m->w_logits, D, m->V, cur, &m->t_w_logits);
+  if (rc == MT3_OK) {
+    const cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "teacher-forced weight prep -> %s", cudaGetErrorString(e));
+  }
+  if (rc != MT3_OK) {
+    cudaFree(slab);
+    return rc;
+  }
+  m->slab_tf = slab;
+  return MT3_OK;
+}
+
+// an activation [rows, cols] of the pass (lo null unless TF32X3); on the wgmma path also its TMA operand
+static int tf_act(const Model* m, float* hi, float* lo, int64_t rows, int cols, Act* a, uint32_t box_rows = 128) {
+  a->hi = hi; a->lo = lo;
+  return m->tc ? make_operand(&a->op, hi, lo, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, box_rows) : MT3_OK;
+}
+
+static int teacher_forced_impl(Model* m, const float* encoded, int B, int T, const int* tok_in, const int* tgt, const int* wts, int L,
+                               float* logits, float* scores, char* ws, cudaStream_t s) {
+  const int Lp = tf_pad(L), D = m->D, Q = m->Q, F = m->F, V = m->V, H = m->H;
+  const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T;
+  const bool s3 = m->split3, tcs = tf_self_tc(m), tcc = tf_cross_tc(m, T);
+  const TfLayout w = tf_layout(m, B, T, L);
+  auto P = [&](int64_t off, bool on = true) { return on ? (float*)(ws + off) : nullptr; };
+  Act y, qkv, vt, ao, qc, enc, ckv, cvt, g;
+  MT3_TRY(tf_act(m, P(w.y), P(w.y_lo, s3), M, D, &y));
+  MT3_TRY(tf_act(m, P(w.ao), P(w.ao_lo, s3), M, Q, &ao));
+  MT3_TRY(tf_act(m, P(w.g), P(w.g_lo, s3), M, F, &g));
+  MT3_TRY(tf_act(m, P(w.qkv), P(w.qkv_lo, s3 && tcs), M, 3 * Q, &qkv));
+  MT3_TRY(tf_act(m, P(w.qc), P(w.qc_lo, s3 && tcc), M, Q, &qc));
+  MT3_TRY(tf_act(m, P(w.ckv), P(w.ckv_lo, s3 && tcc), Me, 2 * Q, &ckv));
+  if (tcs) MT3_TRY(tf_act(m, P(w.vt), P(w.vt_lo, s3), (int64_t)B * H * 64, Lp, &vt, 64));
+  if (tcc) MT3_TRY(tf_act(m, P(w.cvt), P(w.cvt_lo, s3), (int64_t)B * H * 64, T, &cvt, 64));
+  if (s3) {
+    const long long n4 = Me * D / 4;
+    split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(encoded, P(w.enc), P(w.enc_lo), n4);
+    MT3_LAUNCH_CHECK();
+    MT3_TRY(tf_act(m, P(w.enc), P(w.enc_lo), Me, D, &enc));
+  } else {
+    MT3_TRY(tf_act(m, const_cast<float*>(encoded), nullptr, Me, D, &enc));
+  }
+  float* rstd = P(w.rstd);
+  float* scratch = P(w.scratch, w.logits > w.scratch);
+  auto norm = [&]() { return launch_row_rstd(y.hi, y.lo, D, (int)M, D, 1e-6f, rstd, s); };
+  auto residual = [&](const Act& A, int K, const float* wt, const TcW& tw) {     // y += A . W
+    TcGemmArgs a = gemm_epi((int)M, D, K, y.hi, y.lo, D);
+    a.epi = EPI_RESIDUAL; a.R_hi = y.hi; a.R_lo = y.lo; a.ldr = D;
+    return enc_gemm(m, A, wt, tw, a, s);
+  };
+
+  MT3_TRY(launch_embed_seq(tok_in, B, L, Lp, m->emb, D, V, m->pe, y.hi, y.lo, s));
+  for (int l = 0; l < m->Ld; ++l) {
+    const DecLayer& dl = m->dec[l];
+    // self-attention: RMSNorm folded into the QKV projection's row scale; mask make_decoder_mask(targets)
+    MT3_TRY(norm());
+    {
+      TcGemmArgs a = gemm_epi((int)M, 3 * Q, D, qkv.hi, qkv.lo, 3 * Q);
+      a.row_scale = rstd;
+      if (tcs) { a.VT_hi = vt.hi; a.VT_lo = vt.lo; a.vt_col0 = 2 * Q; a.vt_T = Lp; a.vt_H = H; }
+      MT3_TRY(enc_gemm(m, y, dl.wqkv, dl.t_wqkv, a, s));
+    }
+    if (tcs) MT3_TRY(launch_attention_tc(qkv.op, 0, Lp, qkv.op, Q, Lp, vt.op, B, H, ao.hi, ao.lo, s3, true, tgt, L, s, scratch));
+    else MT3_TRY(launch_attention_fp32(qkv.hi, 3 * Q, 0, qkv.hi, 3 * Q, Q, 2 * Q, Lp, Lp, H, B, ao.hi, ao.lo, Q, tgt, L, s));
+    MT3_TRY(residual(ao, Q, dl.wo, dl.t_wo));
+    // cross-attention over all T encoder positions; K/V projected from `encoded` for this layer
+    MT3_TRY(norm());
+    {
+      TcGemmArgs a = gemm_epi((int)M, Q, D, qc.hi, qc.lo, Q);
+      a.row_scale = rstd;
+      MT3_TRY(enc_gemm(m, y, dl.wq_c, dl.t_wq_c, a, s));
+    }
+    {
+      TcGemmArgs a = gemm_epi((int)Me, 2 * Q, D, ckv.hi, ckv.lo, 2 * Q);
+      if (tcc) { a.VT_hi = cvt.hi; a.VT_lo = cvt.lo; a.vt_col0 = Q; a.vt_T = T; a.vt_H = H; }
+      MT3_TRY(enc_gemm(m, enc, dl.wkv_c, dl.t_wkv_c, a, s));
+    }
+    if (tcc) MT3_TRY(launch_attention_tc(qc.op, 0, Lp, ckv.op, 0, T, cvt.op, B, H, ao.hi, ao.lo, s3, false, nullptr, 0, s, scratch));
+    else MT3_TRY(launch_attention_fp32(qc.hi, Q, 0, ckv.hi, 2 * Q, 0, Q, Lp, T, H, B, ao.hi, ao.lo, Q, nullptr, 0, s));
+    MT3_TRY(residual(ao, Q, dl.wo_c, dl.t_wo_c));
+    // gated-GELU MLP
+    MT3_TRY(norm());
+    {
+      TcGemmArgs a = gemm_epi((int)M, 2 * F, D, g.hi, g.lo, F);
+      a.row_scale = rstd; a.epi = EPI_GATED_GELU;
+      MT3_TRY(enc_gemm(m, y, dl.wi, dl.t_wi, a, s));
+    }
+    MT3_TRY(residual(g, F, dl.wo2, dl.t_wo2));
+  }
+  // decoder_norm (folded into w_logits) + logits_dense, then the scores, in chunks of rows
+  MT3_TRY(norm());
+  float* chunk = P(w.logits);
+  for (int64_t r0 = 0; r0 < M; r0 += kTfLogitRows) {
+    const int n = (int)std::min((int64_t)kTfLogitRows, M - r0);
+    Act ys;
+    MT3_TRY(tf_act(m, y.hi + r0 * D, y.lo ? y.lo + r0 * D : nullptr, n, D, &ys));
+    TcGemmArgs a = gemm_epi(n, V, D, chunk, nullptr, V);
+    a.row_scale = rstd + r0;
+    MT3_TRY(enc_gemm(m, ys, m->w_logits, m->t_w_logits, a, s));
+    MT3_TRY(launch_token_score(chunk, V, (int)r0, n, Lp, L, tgt, wts, scores, logits, s));
+  }
+  return MT3_OK;
+}
+
 }  // namespace mt3
 
 using namespace mt3;
@@ -752,6 +936,7 @@ extern "C" int mt3_model_destroy(mt3_model* h) {
   if (m->h_flag) cudaFreeHost(m->h_flag);
   cudaFree(m->slab);
   cudaFree(m->slab_tc);
+  cudaFree(m->slab_tf);
   delete m;
   return MT3_OK;
 }
@@ -951,6 +1136,44 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
   MT3_CUDA_CHECK(cudaMemcpyAsync(tokens_out, m->tokens, (size_t)m->B * m->L * sizeof(int), cudaMemcpyDeviceToDevice, s));
   if (steps_run) *steps_run = ran;
   return MT3_OK;
+}
+
+extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length, int32_t target_length) {
+  if (!h) return -1;
+  const Model* m = reinterpret_cast<const Model*>(h);
+  if (batch <= 0 || batch > m->cfg.max_batch || input_length <= 0 || input_length > m->cfg.max_input_length || target_length <= 0 ||
+      target_length > m->L)
+    return -1;
+  return tf_layout(m, batch, input_length, target_length).total;
+}
+
+extern "C" int mt3_decode_teacher_forced(mt3_model* h, const float* encoded, int32_t batch, int32_t input_length,
+                                         const int32_t* decoder_input_tokens, const int32_t* decoder_target_tokens,
+                                         const int32_t* loss_weights, int32_t target_length, float* logits, float* token_scores,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+  MT3_REQUIRE(h && encoded && decoder_input_tokens && decoder_target_tokens, MT3_ERR_BAD_ARG, "mt3_decode_teacher_forced: null argument");
+  MT3_REQUIRE(logits || token_scores, MT3_ERR_BAD_ARG, "mt3_decode_teacher_forced: logits and token_scores are both NULL");
+  MT3_REQUIRE(((uintptr_t)logits & 15) == 0, MT3_ERR_BAD_ARG, "mt3_decode_teacher_forced: logits must be 16-byte aligned");
+  Model* m = reinterpret_cast<Model*>(h);
+  MT3_REQUIRE(batch > 0 && batch <= m->cfg.max_batch, MT3_ERR_SHAPE, "batch %d outside (0, max_batch=%d]", batch, m->cfg.max_batch);
+  MT3_REQUIRE(input_length > 0 && input_length <= m->cfg.max_input_length, MT3_ERR_SHAPE,
+              "input_length %d outside (0, max_input_length=%d]", input_length, m->cfg.max_input_length);
+  MT3_REQUIRE(target_length > 0 && target_length <= m->L, MT3_ERR_SHAPE, "target_length %d outside (0, max_decode_length=%d]",
+              target_length, m->L);
+  MT3_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, MT3_ERR_WORKSPACE, "workspace must be non-null and 256-byte aligned");
+  const TfLayout w = tf_layout(m, batch, input_length, target_length);
+  MT3_REQUIRE(workspace_bytes >= w.total, MT3_ERR_WORKSPACE, "workspace has %lld bytes, %lld needed", (long long)workspace_bytes,
+              (long long)w.total);
+  // the exact-fp32 attention kernel's limit where it runs, and the wgmma GEMM's N tiling of the logits projection
+  MT3_REQUIRE(tf_self_tc(m) || enc_attention_smem(tf_pad(target_length)) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED,
+              "mt3_decode_teacher_forced: target_length %d too long for the exact-fp32 attention kernel", target_length);
+  MT3_REQUIRE(tf_cross_tc(m, input_length) || enc_attention_smem(input_length) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED,
+              "mt3_decode_teacher_forced: input_length %d too long for the exact-fp32 attention kernel", input_length);
+  MT3_REQUIRE(!m->tc || m->V % 32 == 0, MT3_ERR_UNSUPPORTED, "mt3_decode_teacher_forced: the wgmma logits GEMM needs vocab %% 32 == 0");
+  cudaStream_t s = (cudaStream_t)stream;
+  MT3_TRY(ensure_tf_weights(m, s));
+  return teacher_forced_impl(m, encoded, batch, input_length, decoder_input_tokens, decoder_target_tokens, loss_weights, target_length, logits,
+                             token_scores, (char*)workspace, s);
 }
 
 extern "C" int mt3_vocab_decode(const int32_t* ids, int32_t batch, int32_t length, int32_t num_regular_tokens, int32_t* out,

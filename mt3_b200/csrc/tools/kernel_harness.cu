@@ -101,6 +101,38 @@ KH_API int kh_enc_attention_fp32(const float* qkv, int B, int T, int H, float* o
   return launch_enc_attention(qkv, 3 * H * 64, T, H, B, out, out_lo, H * 64, 0);
 }
 
+// The teacher-forced decoder's attention forms.  q [B*Tq, ldq] (head h at columns q_col0 + 64 h), k [B*Tk, ldk] (k_col0),
+// hi and lo; vt [B*H*64, Tk] (keys in vt_key_slot() order); out [B*Tq, H*64].  causal: Tq = Tk (a multiple of 128) and
+// key_valid [B, n_valid]; otherwise every key is visible.
+KH_API int kh_attention_tc(const float* q_hi, const float* q_lo, int ldq, int q_col0, int Tq, const float* k_hi, const float* k_lo, int ldk,
+                           int k_col0, int Tk, const float* vt_hi, const float* vt_lo, int B, int H, float* out_hi, float* out_lo, int split3,
+                           int causal, const int* key_valid, int n_valid, float* scratch) {
+  TcOperand oq, ok, ov;
+  int r = make_operand(&oq, q_hi, q_lo, (uint64_t)B * Tq, (uint64_t)ldq, (uint64_t)ldq);
+  if (r != MT3_OK) return r;
+  r = make_operand(&ok, k_hi, k_lo, (uint64_t)B * Tk, (uint64_t)ldk, (uint64_t)ldk);
+  if (r != MT3_OK) return r;
+  r = make_operand(&ov, vt_hi, vt_lo, (uint64_t)B * H * 64, (uint64_t)Tk, (uint64_t)Tk, 64);
+  if (r != MT3_OK) return r;
+  return launch_attention_tc(oq, q_col0, Tq, ok, k_col0, Tk, ov, B, H, out_hi, out_lo, split3 != 0, causal != 0, key_valid, n_valid, 0,
+                             scratch);
+}
+KH_API long long kh_attention_tc_scratch_floats(int B, int Tq, int Tk, int H, int causal) {
+  return (long long)attention_tc_scratch_floats(B, Tq, Tk, H, causal != 0);
+}
+
+// the exact-fp32 forms: q [B*Tq, ldq], kv [B*Tk, ldkv] (keys at k_col0, values at v_col0); causal iff key_valid != null
+KH_API int kh_attention_fp32(const float* q, int ldq, int q_col0, const float* kv, int ldkv, int k_col0, int v_col0, int Tq, int Tk, int H,
+                             int B, float* out, float* out_lo, const int* key_valid, int n_valid) {
+  return launch_attention_fp32(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, B, out, out_lo, H * 64, key_valid, n_valid, 0);
+}
+
+// token scores of logits rows row0 .. row0 + n_rows - 1 of [B * Lp] (logits [n_rows, V])
+KH_API int kh_token_score(const float* logits, int V, int row0, int n_rows, int Lp, int L, const int* target, const int* weight,
+                          float* scores, float* logits_out) {
+  return launch_token_score(logits, V, row0, n_rows, Lp, L, target, weight, scores, logits_out, 0);
+}
+
 KH_API int kh_dec_gemm_cluster(const DecGemmArgs* a) { return launch_dec_gemm_cluster(*a, false, 0); }
 KH_API int kh_dec_gemm(const DecGemmArgs* a) { return launch_dec_gemm(*a, 0); }
 KH_API int kh_dec_gemm_out_q(const DecGemmArgs* a0, const DecGemmArgs* a1) { return launch_dec_gemm_out_q(*a0, *a1, false, 0); }

@@ -27,9 +27,32 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
-from . import _lib, gin_lite, network, note_decoding, spectrograms, vocabularies, weights
+from . import _lib, gin_lite, models, network, note_decoding, note_encoding, spectrograms, vocabularies, weights
 
 _GIN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "gin")
+
+
+def segment_score_targets(note_sequence, codec, vocabulary, frame_times, inputs_length: int, encoding_spec: str,
+                          targets_length: int = 1024) -> Dict[str, np.ndarray]:
+    """The decoder features of every audio segment's labels, built the way the transcription tasks and the feature
+    converter build them: note_sequence_to_segment_targets per segment of `inputs_length` frames (ties for
+    NoteEncodingWithTiesSpec, onsets only for NoteOnsetEncodingSpec), the vocabulary's +3 offset, EOS appended
+    (tasks.py:179, seqio's tokenize_and_append_eos), then trimmed or zero-padded to `targets_length` with the decoder input
+    shifted right behind a 0 (models.py:77-98).  Returns int32 [S, targets_length] arrays 'decoder_input_tokens',
+    'decoder_target_tokens', 'decoder_loss_weights'.  Host only."""
+    segs = note_encoding.note_sequence_to_segment_targets(
+        note_sequence, codec, frame_times, inputs_length, onsets_only=encoding_spec == 'NoteOnsetEncodingSpec',
+        include_ties=encoding_spec == 'NoteEncodingWithTiesSpec')
+    conv = models.ContinuousInputsEncDecFeatureConverter()
+    keys = ('decoder_input_tokens', 'decoder_target_tokens', 'decoder_loss_weights')
+    out = {k: np.zeros((len(segs), targets_length), np.int32) for k in keys}
+    for i, toks in enumerate(segs):
+        targets = np.asarray(list(vocabulary.encode(toks)) + [1], np.int32)        # EOS = 1 (vocabularies.py:157-159)
+        feats = conv.convert_example({'inputs': np.zeros((0, 1), np.float32), 'targets': targets},
+                                     {'inputs': 0, 'targets': targets_length})
+        for k in keys:
+            out[k][i] = feats[k]
+    return out
 
 
 class InferenceModel(object):
@@ -234,6 +257,44 @@ class InferenceModel(object):
         # shard of the segments and receives all token streams after one all-gather; identity with a single process
         tokens = self.transcribe_segments_sharded(segs, n_valid_frames=n_valid)
         return [self.postprocess(t, ex) for t, ex in zip(tokens, ds)]
+
+    def score(self, audio, note_sequence) -> List[Dict]:
+        """Log-likelihood of a labelled transcription given the audio, per segment: T5X score_batch over the segments the
+        notebook's preprocessing cuts (same audio path as predict_segments: GPU log-mel with the valid-frame count, padding
+        to inputs_length, encode; batches of batch_size), with targets from segment_score_targets.  Returns one dict per
+        segment: 'start_time' (as postprocess rounds it), 'score' (sum of the token scores), 'num_tokens' (scored
+        positions), 'token_scores' float32 [1024]."""
+        frames, frame_times = self._audio_to_frames(audio)
+        ds = self.preprocess([{'inputs': frames, 'input_times': frame_times}])
+        tg = segment_score_targets(note_sequence, self.codec, self.vocabulary, frame_times, self.inputs_length,
+                                   self.encoding_spec, self.outputs_length)
+        if len(tg['decoder_target_tokens']) != len(ds):
+            raise RuntimeError('segment count mismatch: %d target segments, %d audio segments'
+                               % (len(tg['decoder_target_tokens']), len(ds)))
+        hop = self.spectrogram_config.hop_width
+        segs = np.zeros((len(ds), self.inputs_length * hop), np.float32)
+        n_valid = np.zeros((len(ds),), np.int32)
+        for i, ex in enumerate(ds):
+            flat = np.asarray(ex['inputs'], np.float32).reshape(-1)
+            segs[i, :flat.size] = flat
+            n_valid[i] = flat.size // hop
+        scores = np.zeros((len(ds), self.outputs_length), np.float32)
+        nv = torch.from_numpy(n_valid).to(self.device)
+        for s0 in range(0, len(ds), self.batch_size):
+            s1 = min(len(ds), s0 + self.batch_size)
+            dev = torch.from_numpy(segs[s0:s1]).to(self.device)
+            spec = self._pad_inputs(spectrograms.compute_spectrogram(dev, self.spectrogram_config, n_valid_frames=nv[s0:s1]))
+            encoded = self.model.encode(spec)
+            ts = self.model.score(encoded, tg['decoder_input_tokens'][s0:s1], tg['decoder_target_tokens'][s0:s1],
+                                  tg['decoder_loss_weights'][s0:s1])
+            scores[s0:s1] = ts.cpu().numpy()
+        out = []
+        for i, ex in enumerate(ds):
+            start_time = ex['input_times'][0]
+            start_time -= start_time % (1 / self.codec.steps_per_second)
+            out.append({'start_time': start_time, 'score': float(scores[i].astype(np.float64).sum()),
+                        'num_tokens': int(tg['decoder_loss_weights'][i].sum()), 'token_scores': scores[i]})
+        return out
 
     # ---------------------------------------------------------------------------------
     # Batch inference over many recordings (T5X `infer` with gin/infer.gin + inference.write_inferences_to_file)

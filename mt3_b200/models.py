@@ -8,7 +8,9 @@ behind a 0 and the loss weights mark the non-padding targets.  seqio's packing i
 `ContinuousInputsEncoderDecoderModel` (models.py:121-152) pairs a `network.Transformer` with the converter and a decode
 function: `predict_batch` is T5X's predict_batch_with_aux at num_decodes = 1 (BOS 0, EOS 1, at most max_decode_length
 steps) -- `decode_fn='beam_search'` is the reference's default (models.py:127) and runs the library's beam-size-1
-bookkeeping, `decode_fn='greedy'` the plain argmax loop.  Training (loss, optimizer, label smoothing) is out of scope.
+bookkeeping, `decode_fn='greedy'` the plain argmax loop.  `score_batch` is T5X's EncoderDecoderModel.score_batch (which
+the reference's model inherits): the log-likelihood of given targets, from the teacher-forced decoder pass.  Training
+(loss, optimizer, label smoothing) is out of scope.
 """
 from __future__ import annotations
 
@@ -107,3 +109,22 @@ class ContinuousInputsEncoderDecoderModel:
 
     def predict_batch(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None):
         return self.predict_batch_with_aux(params, batch, rng=rng, decoder_params=decoder_params)[0]
+
+    def score_batch(self, params, batch: Mapping[str, Any], return_intermediates: bool = False):
+        """T5X EncoderDecoderModel.score_batch with z_loss = 0: float32 [B], the sum over positions of
+        (log_softmax(logits)[target] * decoder_loss_weights).  `batch` holds the model features of the feature converter
+        (encoder_input_tokens, decoder_input_tokens, decoder_target_tokens, decoder_loss_weights), numpy or torch.
+        `params` is accepted for signature fidelity: the weights live in the module."""
+        del params
+        if return_intermediates:
+            raise ValueError('return_intermediates=True is not supported: the pass keeps no intermediates')
+        import torch
+        x = batch['encoder_input_tokens']
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x, np.float32))
+        if x.shape[-1] != self._input_depth:
+            raise ValueError('encoder_input_tokens depth %d != input_depth %d' % (x.shape[-1], self._input_depth))
+        encoded = self.module.encode(x.to(self.module.device))
+        token_scores = self.module.score(encoded, batch['decoder_input_tokens'], batch['decoder_target_tokens'],
+                                         batch.get('decoder_loss_weights'))
+        return token_scores.to(torch.float64).sum(-1).to(torch.float32)

@@ -1,8 +1,9 @@
 """T5-style encoder/decoder of MT3 on sm_90a: the reference's network.py surface.
 
-`T5Config` mirrors network.py:25-41; `Transformer` exposes encode / decode (single-step,
-decode=True) like the Flax module (network.py:265-361), plus `generate`, which stands in
-for t5x's predict_batch_with_aux at num_decodes=1 (models.py:121-138).  All compute runs in
+`T5Config` mirrors network.py:25-41; `Transformer` exposes encode, decode -- one step (decode=True) or the
+teacher-forced pass over a whole target sequence (decode=False) -- and __call__ like the Flax module (network.py:265-409),
+plus `score` (the token scores of T5X's score_batch) and `generate`, which stands in for t5x's predict_batch_with_aux at
+num_decodes=1 (models.py:121-138).  All compute runs in
 libmt3b200.so; tensors are only the memory container.  Drop-in boundary B3 (SURVEY.md 8b).
 """
 from __future__ import annotations
@@ -70,6 +71,7 @@ class Transformer:
         self._h = h
         self._ws = None
         self._ws_key = None
+        self._tf_ws = None              # workspace of the teacher-forced pass (its own: the decode state stays untouched)
 
     # -- plumbing ---------------------------------------------------------------------
     def __del__(self):
@@ -131,12 +133,22 @@ class Transformer:
     def decode(self, encoded, encoder_input_tokens, decoder_input_tokens, decoder_target_tokens=None,
                encoder_segment_ids=None, decoder_segment_ids=None, decoder_positions=None, enable_dropout=False,
                decode=True, max_decode_length=None):
-        """One Transformer.decode(decode=True) step (network.py:303-361): decoder_input_tokens
-        int32 [B,1] -> logits float32 [B,1,V]; the KV cache lives in the model handle
-        (call init_cache(encoded) first).  The teacher-forced decode=False form is training-only."""
+        """Transformer.decode (network.py:303-361).
+        decode=True: one step, decoder_input_tokens int32 [B,1] -> logits float32 [B,1,V]; the KV cache lives in the model
+        handle (call init_cache(encoded) first).
+        decode=False: the teacher-forced pass over all L positions, decoder_input_tokens / decoder_target_tokens [B,L] ->
+        logits float32 [B,L,V], with the self-attention mask make_decoder_mask(decoder_target_tokens).  Positions with
+        target 0 (padding) get finite values that differ from the reference's (DESIGN.md section 1).  Touches no decode
+        state."""
         if not decode:
-            raise NotImplementedError("decode=False (teacher-forced training pass) is out of scope; "
-                                      "use teacher_forced_logits for evaluation")
+            if enable_dropout:
+                raise ValueError("inference only: enable_dropout must be False")
+            if encoder_segment_ids is not None or decoder_segment_ids is not None:
+                raise ValueError("packing (segment ids) is a training feature; not on this path")
+            if decoder_target_tokens is None:
+                raise ValueError("decode=False needs decoder_target_tokens (they make the self-attention mask)")
+            del decoder_positions       # the reference ignores them too: positions are arange(L) (network.py:211-217)
+            return self._teacher_forced(encoded, decoder_input_tokens, decoder_target_tokens, None, True, False)[0]
         if encoder_segment_ids is not None:
             raise ValueError('During decoding, packing should not be used but `encoder_segment_ids` was passed '
                              'to `Transformer.decode`.')
@@ -153,6 +165,74 @@ class Transformer:
         with torch.cuda.device(self.device):
             _lib.check(self._lib.mt3_decode_step(self._h, tok.data_ptr(), logits.data_ptr(), None, self._stream()))
         return logits
+
+    def __call__(self, encoder_input_tokens, decoder_input_tokens, decoder_target_tokens, encoder_segment_ids=None,
+                 decoder_segment_ids=None, encoder_positions=None, decoder_positions=None, *, enable_dropout: bool = False,
+                 decode: bool = False):
+        """Transformer.__call__ (network.py:363-409): encode, then decode(decode=False) -> logits float32 [B,L,V]."""
+        del encoder_positions
+        encoded = self.encode(encoder_input_tokens, encoder_segment_ids=encoder_segment_ids, enable_dropout=enable_dropout)
+        return self.decode(encoded, encoder_input_tokens, decoder_input_tokens, decoder_target_tokens,
+                           encoder_segment_ids=encoder_segment_ids, decoder_segment_ids=decoder_segment_ids,
+                           decoder_positions=decoder_positions, enable_dropout=enable_dropout, decode=decode)
+
+    def score(self, encoded: torch.Tensor, decoder_input_tokens, decoder_target_tokens, decoder_loss_weights=None) -> torch.Tensor:
+        """Token scores float32 [B,L] of T5X's score_batch (z_loss 0): (logits[target] - logsumexp(logits)) * weight, weight
+        = decoder_loss_weights or target > 0.  The logits are not materialised: they go through the library's workspace in
+        chunks of rows."""
+        return self._teacher_forced(encoded, decoder_input_tokens, decoder_target_tokens, decoder_loss_weights, False, True)[1]
+
+    def _tokens(self, t, name: str, shape=None) -> torch.Tensor:
+        if isinstance(t, np.ndarray):
+            t = torch.from_numpy(t)
+        if not isinstance(t, torch.Tensor) or t.dtype not in (torch.int32, torch.int64, torch.int16, torch.uint8):
+            raise ValueError(f'{name}: input type must be an integer or unsigned integer.')   # layers.py:528-529
+        if t.dim() != 2:
+            raise ValueError(f'{name} must be [batch, length]; got shape {tuple(t.shape)}')
+        if shape is not None and tuple(t.shape) != shape:
+            raise ValueError(f'{name} has shape {tuple(t.shape)}, expected {shape}')
+        return t.to(device=self.device, dtype=torch.int32).contiguous()
+
+    def _teacher_forced(self, encoded, decoder_input_tokens, decoder_target_tokens, decoder_loss_weights, want_logits: bool,
+                        want_scores: bool):
+        """mt3_decode_teacher_forced: (logits [B,L,V] or None, token scores [B,L] or None)."""
+        if not (isinstance(encoded, torch.Tensor) and encoded.is_cuda and encoded.dtype == torch.float32 and encoded.dim() == 3):
+            raise TypeError("encoded must be a CUDA float32 tensor [batch, input_length, emb_dim]")
+        if encoded.shape[-1] != self.config.emb_dim:
+            raise ValueError(f"encoded width {encoded.shape[-1]} != emb_dim {self.config.emb_dim}")
+        b, t, _ = encoded.shape
+        tok_in = self._tokens(decoder_input_tokens, 'decoder_input_tokens')
+        length = tok_in.shape[1]
+        tgt = self._tokens(decoder_target_tokens, 'decoder_target_tokens', (b, length))
+        wts = None if decoder_loss_weights is None else self._tokens(decoder_loss_weights, 'decoder_loss_weights', (b, length))
+        if tok_in.shape[0] != b:
+            raise ValueError(f'decoder tokens have batch {tok_in.shape[0]}, encoded has {b}')
+        if not 0 < length <= self.max_decode_length:
+            raise ValueError(f'decoder length {length} outside (0, max_decode_length={self.max_decode_length}]')
+        if not 0 < b <= self._cfg.max_batch:
+            raise ValueError(f'batch {b} outside (0, max_batch={self._cfg.max_batch}]')
+        if not 0 < t <= self._cfg.max_input_length:
+            raise ValueError(f'input length {t} outside (0, max_input_length={self._cfg.max_input_length}]')
+        v = self.config.vocab_size
+        for name, x in (('decoder_input_tokens', tok_in), ('decoder_target_tokens', tgt)):
+            lo, hi = int(x.min()), int(x.max())
+            if lo < 0 or hi >= v:
+                raise ValueError(f'{name}: ids must lie in [0, vocab_size={v}); got [{lo}, {hi}]')
+        nbytes = int(self._lib.mt3_teacher_forced_workspace_bytes(self._h, b, t, length))
+        if nbytes <= 0:
+            raise _lib.Mt3Error(-2, f"no teacher-forced workspace layout for batch={b}, input_length={t}, length={length}")
+        if self._tf_ws is None or self._tf_ws.numel() < nbytes:
+            self._tf_ws = None
+            self._tf_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        logits = torch.empty((b, length, v), dtype=torch.float32, device=self.device) if want_logits else None
+        scores = torch.empty((b, length), dtype=torch.float32, device=self.device) if want_scores else None
+        enc = encoded.contiguous()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.mt3_decode_teacher_forced(
+                self._h, enc.data_ptr(), b, t, tok_in.data_ptr(), tgt.data_ptr(), None if wts is None else wts.data_ptr(), length,
+                None if logits is None else logits.data_ptr(), None if scores is None else scores.data_ptr(),
+                self._tf_ws.data_ptr(), self._tf_ws.numel(), self._stream()))
+        return logits, scores
 
     # -- helpers built on the step ----------------------------------------------------
     def teacher_forced_logits(self, encoded: torch.Tensor, decoder_input_tokens: torch.Tensor) -> torch.Tensor:
