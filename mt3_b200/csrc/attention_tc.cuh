@@ -1,5 +1,5 @@
-// K4: encoder self-attention on the Hopper tensor cores (wgmma + TMA), sm_90a; the same work loop also runs the
-// teacher-forced decoder's causal self-attention and cross-attention (attention_tc_kernel, launch_attention_tc).
+// K4: attention on the Hopper tensor cores (wgmma + TMA), sm_90a: the encoder's self-attention and the teacher-forced
+// decoder's causal self-attention and cross-attention (attention_tc_kernel, launch_attention_tc).
 //
 // Reference: dot_product_attention (layers.py:85-157): softmax_k(q . k^T) . v, logits NOT scaled by
 // 1/sqrt(d) (layers.py:230-234), mask all ones in the encoder (network.py:283-289).
@@ -124,7 +124,7 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Mask kinds of the attention body.  NONE: every key below the item's key count is visible (encoder, cross-attention).
+// Mask kinds of the attention kernel.  NONE: every key below the item's key count is visible (encoder, cross-attention).
 // CAUSAL: query i sees key j iff j <= i, j < n_valid and key_valid[b][j] > 0 (the teacher-forced decoder's
 // make_decoder_mask); a row whose every key is masked writes 0.
 constexpr int kAtMaskNone = 0, kAtMaskCausal = 1;
@@ -143,7 +143,6 @@ __device__ __forceinline__ void at_chunk_mask(float (&s)[64], int j0, int i0, co
     }
 }
 
-// The attention work loop, shared by the encoder kernel and the decoder's teacher-forced kernels.
 // PERSISTENT: one CTA per SM walks over work items (sequence b, head h, 128-query tile) with stride gridDim.x.  All
 // mbarriers complete exactly once per item, so the wait parity is (item counter & 1).  The TMA thread streams ahead of
 // the consumers: Q of item i+1 as soon as both warpgroups have finished S(i), K of item i+1 as soon as they have
@@ -152,13 +151,16 @@ __device__ __forceinline__ void at_chunk_mask(float (&s)[64], int j0, int i0, co
 // Q of head h: columns q_col0 + 64 h of the rows [b Tq, (b + 1) Tq) of tq_*; K: columns k_col0 + 64 h of the rows
 // [b Tk, (b + 1) Tk) of tk_*.  Under CAUSAL the items of key parts that lie wholly above the diagonal are skipped (the
 // item counter does not advance for them, in the producer and the consumers alike).
-// PSPLIT: P . V in 3xTF32 too (P_hi V_hi + P_hi V_lo + P_lo V_hi, P kept in fp32) instead of P rounded to tf32.
-template <bool SPLIT3, bool KSPLIT, int NCHUNK, int MASK, bool PSPLIT = false>
-__device__ __forceinline__ void attention_tc_body(const CUtensorMap* tq_hi, const CUtensorMap* tq_lo, const CUtensorMap* tk_hi,
-                                                  const CUtensorMap* tk_lo, const CUtensorMap* tv_hi, const CUtensorMap* tv_lo,
-                                                  int q_col0, int k_col0, int Tq, int Tk, int H, int B, float* __restrict__ out_hi,
-                                                  float* __restrict__ out_lo, int ldo, int TK_arg, int KS_arg, float* __restrict__ part_o,
-                                                  float2* __restrict__ part_ml, const int* __restrict__ key_valid, int n_valid) {
+// PSPLIT: P . V in 3xTF32 too (P_hi V_hi + P_hi V_lo + P_lo V_hi, P kept in fp32) instead of P rounded to tf32.  The
+// teacher-forced pass splits P so that the decoder's logits stay within the float32 bar of DESIGN.md section 4 (P rounded
+// to tf32 moves them by about 1e-4 of their scale); the encoder rounds P, and its accuracy bar and speed were measured so.
+template <bool SPLIT3, bool KSPLIT, int NCHUNK, int MASK, bool PSPLIT>
+__global__ void __launch_bounds__(kAtThreads, 1)
+attention_tc_kernel(const __grid_constant__ CUtensorMap tq_hi, const __grid_constant__ CUtensorMap tq_lo,
+                    const __grid_constant__ CUtensorMap tk_hi, const __grid_constant__ CUtensorMap tk_lo,
+                    const __grid_constant__ CUtensorMap tv_hi, const __grid_constant__ CUtensorMap tv_lo, int q_col0, int k_col0, int Tq,
+                    int Tk, int H, int B, float* __restrict__ out_hi, float* __restrict__ out_lo, int ldo, int TK_arg, int KS_arg,
+                    float* __restrict__ part_o, float2* __restrict__ part_ml, const int* __restrict__ key_valid, int n_valid) {
   const int KS = KSPLIT ? KS_arg : 1, TK = KSPLIT ? TK_arg : Tk;      // compile-time 1 / Tk in the common single-pass form
   // TK = keys per work item (<= 256), KS = key parts per query tile (Tk <= KS * TK).  KS == 1: the item covers all keys and
   // writes the normalised output.  KS > 1 (T = 512, ismir2021; the decoder's L > 256): an item covers keys
@@ -184,13 +186,13 @@ __device__ __forceinline__ void attention_tc_body(const CUtensorMap* tq_hi, cons
   const uint32_t lo_tiles = SPLIT3 ? 2u : 1u;
 
   if (warp == 8 && lane == 0) {
-    tc::prefetch_tmap(tq_hi);
-    if (tk_hi != tq_hi) tc::prefetch_tmap(tk_hi);
-    tc::prefetch_tmap(tv_hi);
+    tc::prefetch_tmap(&tq_hi);
+    tc::prefetch_tmap(&tk_hi);
+    tc::prefetch_tmap(&tv_hi);
     if (SPLIT3) {
-      tc::prefetch_tmap(tq_lo);
-      if (tk_lo != tq_lo) tc::prefetch_tmap(tk_lo);
-      tc::prefetch_tmap(tv_lo);
+      tc::prefetch_tmap(&tq_lo);
+      tc::prefetch_tmap(&tk_lo);
+      tc::prefetch_tmap(&tv_lo);
     }
     tc::mbar_init(q_full, 1);
     for (int c = 0; c < 2; ++c) {
@@ -217,16 +219,16 @@ __device__ __forceinline__ void attention_tc_body(const CUtensorMap* tq_hi, cons
         // Q: the region is free since the previous item's S MMAs (s_done, waited for before that item's V was loaded)
         tc::mbar_arrive_expect_tx(q_full, 2 * lo_tiles * kSubBytes);
         for (int sub = 0; sub < 2; ++sub) {
-          tc::tma_load_2d(sQ + sub * kAtSub, tq_hi, q_full, q_col0 + h * 64 + sub * 32, qrow0 + q0);
-          if (SPLIT3) tc::tma_load_2d(sQ + (2 + sub) * kAtSub, tq_lo, q_full, q_col0 + h * 64 + sub * 32, qrow0 + q0);
+          tc::tma_load_2d(sQ + sub * kAtSub, &tq_hi, q_full, q_col0 + h * 64 + sub * 32, qrow0 + q0);
+          if (SPLIT3) tc::tma_load_2d(sQ + (2 + sub) * kAtSub, &tq_lo, q_full, q_col0 + h * 64 + sub * 32, qrow0 + q0);
         }
         // K chunks -> slots: free once the previous item's P.V MMAs have read V out of them
         if (it > 0) tc::mbar_wait(pv_done, pph);
         for (int c = 0; c < nchunk; ++c) {
           tc::mbar_arrive_expect_tx(&k_full[c], 2 * lo_tiles * kSubBytes);
           for (int sub = 0; sub < 2; ++sub) {
-            tc::tma_load_2d(slot[c] + sub * kAtSub, tk_hi, &k_full[c], k_col0 + h * 64 + sub * 32, krow0 + koff + c * kAtKC);
-            if (SPLIT3) tc::tma_load_2d(slot[c] + (2 + sub) * kAtSub, tk_lo, &k_full[c], k_col0 + h * 64 + sub * 32, krow0 + koff + c * kAtKC);
+            tc::tma_load_2d(slot[c] + sub * kAtSub, &tk_hi, &k_full[c], k_col0 + h * 64 + sub * 32, krow0 + koff + c * kAtKC);
+            if (SPLIT3) tc::tma_load_2d(slot[c] + (2 + sub) * kAtSub, &tk_lo, &k_full[c], k_col0 + h * 64 + sub * 32, krow0 + koff + c * kAtKC);
           }
         }
         // V^T chunks reuse the slots once every S MMA of THIS item has read K
@@ -235,8 +237,8 @@ __device__ __forceinline__ void attention_tc_body(const CUtensorMap* tq_hi, cons
         for (int c = 0; c < nchunk; ++c) {
           tc::mbar_arrive_expect_tx(&v_full[c], 4 * lo_tiles * kVSub);
           for (int sub = 0; sub < 4; ++sub) {
-            tc::tma_load_2d(slot[c] + sub * kVSub, tv_hi, &v_full[c], koff + c * kAtKC + sub * 32, vrow);
-            if (SPLIT3) tc::tma_load_2d(slot[c] + (4 + sub) * kVSub, tv_lo, &v_full[c], koff + c * kAtKC + sub * 32, vrow);
+            tc::tma_load_2d(slot[c] + sub * kVSub, &tv_hi, &v_full[c], koff + c * kAtKC + sub * 32, vrow);
+            if (SPLIT3) tc::tma_load_2d(slot[c] + (4 + sub) * kVSub, &tv_lo, &v_full[c], koff + c * kAtKC + sub * 32, vrow);
           }
         }
       }
@@ -336,36 +338,12 @@ __device__ __forceinline__ void attention_tc_body(const CUtensorMap* tq_hi, cons
   }
 }
 
-// Encoder self-attention: Q, K from one [B*T, 3*H*64] qkv operand, all T keys visible.
-template <bool SPLIT3, bool KSPLIT, int NCHUNK>
-__global__ void __launch_bounds__(kAtThreads, 1)
-enc_attention_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
-                        const __grid_constant__ CUtensorMap tv_hi, const __grid_constant__ CUtensorMap tv_lo, int T, int H, int B,
-                        float* __restrict__ out_hi, float* __restrict__ out_lo, int ldo, int TK_arg, int KS_arg, float* __restrict__ part_o, float2* __restrict__ part_ml) {
-  attention_tc_body<SPLIT3, KSPLIT, NCHUNK, kAtMaskNone>(&tm_hi, &tm_lo, &tm_hi, &tm_lo, &tv_hi, &tv_lo, 0, H * 64, T, T, H, B, out_hi,
-                                                          out_lo, ldo, TK_arg, KS_arg, part_o, part_ml, nullptr, 0);
-}
-
-// The general form: Q and K from separate operands with their own rows per sequence (Tq, Tk), and a mask kind.  With hi/lo
-// operands (TF32X3) P . V is split as well, so that the decoder's logits stay within the float32 bar of DESIGN.md section 4
-// (P rounded to tf32 moves them by about 1e-4 of their scale).
-template <bool SPLIT3, bool KSPLIT, int NCHUNK, int MASK>
-__global__ void __launch_bounds__(kAtThreads, 1)
-attention_tc_kernel(const __grid_constant__ CUtensorMap tq_hi, const __grid_constant__ CUtensorMap tq_lo,
-                    const __grid_constant__ CUtensorMap tk_hi, const __grid_constant__ CUtensorMap tk_lo,
-                    const __grid_constant__ CUtensorMap tv_hi, const __grid_constant__ CUtensorMap tv_lo, int q_col0, int k_col0, int Tq,
-                    int Tk, int H, int B, float* __restrict__ out_hi, float* __restrict__ out_lo, int ldo, int TK_arg, int KS_arg,
-                    float* __restrict__ part_o, float2* __restrict__ part_ml, const int* __restrict__ key_valid, int n_valid) {
-  attention_tc_body<SPLIT3, KSPLIT, NCHUNK, MASK, SPLIT3>(&tq_hi, &tq_lo, &tk_hi, &tk_lo, &tv_hi, &tv_lo, q_col0, k_col0, Tq, Tk, H, B, out_hi,
-                                                  out_lo, ldo, TK_arg, KS_arg, part_o, part_ml, key_valid, n_valid);
-}
-
 // Merge of KS key parts: out[row, h, :] = sum_k e^(m_k - m) O_k / sum_k e^(m_k - m) l_k.  One warp per (row, head).
 // CAUSAL: row t reads only the parts that start at or before t (the others were skipped or are wholly masked for it), a
 // part with no visible key (m_k = -inf) weighs 0, and a row with none at all writes 0.
 template <bool CAUSAL>
-__device__ __forceinline__ void attention_combine_body(const float* __restrict__ part_o, const float2* __restrict__ part_ml, int B, int T,
-                                                       int H, int KS, int TK, float* __restrict__ out_hi, float* __restrict__ out_lo) {
+__global__ void attention_combine_kernel(const float* __restrict__ part_o, const float2* __restrict__ part_ml, int B, int T, int H, int KS,
+                                         int TK, float* __restrict__ out_hi, float* __restrict__ out_lo) {
   const long long item = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);     // (b, t, h)
   const int lane = threadIdx.x & 31;
   if (item >= (long long)B * T * H) return;
@@ -400,95 +378,34 @@ __device__ __forceinline__ void attention_combine_body(const float* __restrict__
   }
 }
 
-__global__ void enc_attention_combine_kernel(const float* __restrict__ part_o, const float2* __restrict__ part_ml, int B, int T, int H,
-                                             int KS, float* __restrict__ out_hi, float* __restrict__ out_lo) {
-  attention_combine_body<false>(part_o, part_ml, B, T, H, KS, 0, out_hi, out_lo);
-}
-__global__ void attention_combine_causal_kernel(const float* __restrict__ part_o, const float2* __restrict__ part_ml, int B, int T, int H,
-                                                int KS, int TK, float* __restrict__ out_hi, float* __restrict__ out_lo) {
-  attention_combine_body<true>(part_o, part_ml, B, T, H, KS, TK, out_hi, out_lo);
-}
-
-// floats of scratch the key-split form needs (T > 256): KS unnormalised O tiles + KS (max, sum) pairs per (row, head)
-inline int64_t enc_attention_tc_scratch_floats(int B, int T, int H) {
-  if (T <= 2 * kAtKC) return 0;
-  const int64_t KS = T / (2 * kAtKC);
-  return KS * (int64_t)B * T * H * 64 + KS * (int64_t)B * H * T * 2;
-}
-inline bool enc_attention_tc_supported(int T) { return T % 8 == 0 && (T <= 2 * kAtKC || T % (2 * kAtKC) == 0); }
-
-// qkv_hi / qkv_lo: [B*T, 3*H*64] (q and k are read); vt: V^T [B*H*64, T] (box rows 64, keys in vt_key_slot() order); out: [B*T, H*64]
-// (out_lo optional).  T <= 256 (T % 8 == 0), or a multiple of 256 (ismir2021: 512) with `scratch`
-// (enc_attention_tc_scratch_floats) for the key-split form.
-inline int launch_enc_attention_tc(const TcOperand& qkv, const TcOperand& vt, int B, int T, int H, float* out_hi, float* out_lo,
-                                   bool split3, cudaStream_t s, float* scratch = nullptr) {
-  MT3_REQUIRE(enc_attention_tc_supported(T), MT3_ERR_UNSUPPORTED, "tc attention: T=%d (needs T <= 256 and a multiple of 8, or a multiple of 256)", T);
-  MT3_REQUIRE(!split3 || qkv.has_lo, MT3_ERR_BAD_ARG, "tc attention: TF32X3 needs hi/lo qkv");
-  const int KS = T <= 2 * kAtKC ? 1 : T / (2 * kAtKC);
-  const int TK = T / KS;
-  const int nchunk = cdiv(TK, kAtKC);
-  MT3_REQUIRE(KS == 1 || scratch != nullptr, MT3_ERR_WORKSPACE, "tc attention: T=%d needs the key-split scratch buffer", T);
-  float* part_o = scratch;
-  float2* part_ml = KS > 1 ? reinterpret_cast<float2*>(scratch + (int64_t)KS * B * T * H * 64) : nullptr;
-  static bool attr_done = false;
-  if (!attr_done) {
-#define MT3_AT_ATTR(S3, KSP, NC) \
-  MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_tc_kernel<S3, KSP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem))
-    MT3_AT_ATTR(true, false, 1); MT3_AT_ATTR(true, false, 2); MT3_AT_ATTR(true, true, 2);
-    MT3_AT_ATTR(false, false, 1); MT3_AT_ATTR(false, false, 2); MT3_AT_ATTR(false, true, 2);
-#undef MT3_AT_ATTR
-    attr_done = true;
-  }
-  static int sm_count = 0;
-  if (!sm_count) {
-    int dev = 0;
-    MT3_CUDA_CHECK(cudaGetDevice(&dev));
-    MT3_CUDA_CHECK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-  }
-  const int n_items = B * H * cdiv(T, kAtQ) * KS;
-  dim3 grid(n_items < sm_count ? n_items : sm_count);       // one persistent CTA per SM (192 KB of shared memory each)
-#define MT3_AT_LAUNCH(S3, KSP, NC, LO_Q, LO_V)                                                                                  \
-  enc_attention_tc_kernel<S3, KSP, NC><<<grid, kAtThreads, kAtSmem, s>>>(qkv.hi, LO_Q, vt.hi, LO_V, T, H, B, out_hi, out_lo, H * 64, TK, \
-                                                                         KS, part_o, part_ml)
-  if (split3 && KS > 1) MT3_AT_LAUNCH(true, true, 2, qkv.lo, vt.lo);
-  else if (split3 && nchunk > 1) MT3_AT_LAUNCH(true, false, 2, qkv.lo, vt.lo);
-  else if (split3) MT3_AT_LAUNCH(true, false, 1, qkv.lo, vt.lo);
-  else if (KS > 1) MT3_AT_LAUNCH(false, true, 2, qkv.hi, vt.hi);
-  else if (nchunk > 1) MT3_AT_LAUNCH(false, false, 2, qkv.hi, vt.hi);
-  else MT3_AT_LAUNCH(false, false, 1, qkv.hi, vt.hi);
-#undef MT3_AT_LAUNCH
-  MT3_LAUNCH_CHECK();
-  if (KS > 1) {
-    const long long items = (long long)B * T * H;
-    enc_attention_combine_kernel<<<(unsigned)((items + 7) / 8), 256, 0, s>>>(part_o, part_ml, B, T, H, KS, out_hi, out_lo);
-    MT3_LAUNCH_CHECK();
-  }
-  return MT3_OK;
-}
-
-// The decoder's teacher-forced forms of the kernel above.  Items of at most 256 keys; the key-split form (parts of 256
-// keys, unnormalised, merged by the combine kernel) when there are more.
+// Items of at most 256 keys; the key-split form (parts of 256 keys, unnormalised, merged by the combine kernel) when there
+// are more.
 //   causal:     Tq = Tk = a multiple of 128 (the sequence padded to the query tile: padded rows come after every real
 //               position, so causality hides them); key j of sequence b is visible to query i iff j <= i, j < n_valid and
 //               key_valid[b * n_valid + j] > 0.  The parts wholly above the diagonal are skipped.
-//   otherwise:  all Tk keys visible to every query (cross-attention: Tk = T, enc_attention_tc_supported(Tk)).
+//   otherwise:  all Tk keys visible to every query (the encoder: Tq = Tk = T; cross-attention: Tk = T); Tk <= 256 and a
+//               multiple of 8, or a multiple of 256 (ismir2021: 512).
 inline int attention_tc_parts(int Tk, bool causal) {
   if (Tk <= 2 * kAtKC) return 1;
   return causal ? cdiv(Tk, 2 * kAtKC) : Tk / (2 * kAtKC);
 }
+// floats of scratch the key-split form needs: KS unnormalised O tiles + KS (max, sum) pairs per (row, head)
 inline int64_t attention_tc_scratch_floats(int B, int Tq, int Tk, int H, bool causal) {
   const int64_t KS = attention_tc_parts(Tk, causal);
   if (KS == 1) return 0;
   return KS * (int64_t)B * Tq * H * 64 + KS * (int64_t)B * H * Tq * 2;
 }
 inline bool attention_tc_supported(int Tq, int Tk, bool causal) {
-  return causal ? (Tq == Tk && Tq % kAtQ == 0) : enc_attention_tc_supported(Tk);
+  if (causal) return Tq == Tk && Tq % kAtQ == 0;
+  return Tk % 8 == 0 && (Tk <= 2 * kAtKC || Tk % (2 * kAtKC) == 0);
 }
 
 // q: an operand whose rows [b Tq, (b + 1) Tq) hold sequence b's queries, head h at columns q_col0 + 64 h; k likewise with
 // Tk and k_col0; vt: V^T [B*H*64, Tk] (box rows 64, keys in vt_key_slot() order); out [B*Tq, H*64] (out_lo optional).
+// split_p: P . V in 3xTF32 as well (the kernel's PSPLIT); ignored unless split3.  scratch: attention_tc_scratch_floats()
+// floats for the key-split form.
 inline int launch_attention_tc(const TcOperand& q, int q_col0, int Tq, const TcOperand& k, int k_col0, int Tk, const TcOperand& vt, int B,
-                               int H, float* out_hi, float* out_lo, bool split3, bool causal, const int* key_valid, int n_valid,
+                               int H, float* out_hi, float* out_lo, bool split3, bool split_p, bool causal, const int* key_valid, int n_valid,
                                cudaStream_t s, float* scratch) {
   MT3_REQUIRE(attention_tc_supported(Tq, Tk, causal), MT3_ERR_UNSUPPORTED, "tc attention: Tq=%d Tk=%d causal=%d is not supported", Tq, Tk,
               (int)causal);
@@ -500,17 +417,6 @@ inline int launch_attention_tc(const TcOperand& q, int q_col0, int Tq, const TcO
   MT3_REQUIRE(KS == 1 || scratch != nullptr, MT3_ERR_WORKSPACE, "tc attention: Tk=%d needs the key-split scratch buffer", Tk);
   float* part_o = scratch;
   float2* part_ml = KS > 1 ? reinterpret_cast<float2*>(scratch + (int64_t)KS * B * Tq * H * 64) : nullptr;
-  static bool attr_done = false;
-  if (!attr_done) {
-#define MT3_AT_ATTR(S3, KSP, NC, MK) \
-  MT3_CUDA_CHECK(cudaFuncSetAttribute(attention_tc_kernel<S3, KSP, NC, MK>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtSmem))
-    MT3_AT_ATTR(true, false, 1, 0); MT3_AT_ATTR(true, false, 2, 0); MT3_AT_ATTR(true, true, 2, 0);
-    MT3_AT_ATTR(false, false, 1, 0); MT3_AT_ATTR(false, false, 2, 0); MT3_AT_ATTR(false, true, 2, 0);
-    MT3_AT_ATTR(true, false, 1, 1); MT3_AT_ATTR(true, true, 2, 1);
-    MT3_AT_ATTR(false, false, 1, 1); MT3_AT_ATTR(false, true, 2, 1);
-#undef MT3_AT_ATTR
-    attr_done = true;
-  }
   static int sm_count = 0;
   if (!sm_count) {
     int dev = 0;
@@ -518,36 +424,37 @@ inline int launch_attention_tc(const TcOperand& q, int q_col0, int Tq, const TcO
     MT3_CUDA_CHECK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
   }
   const int n_items = B * H * cdiv(Tq, kAtQ) * KS;
-  dim3 grid(n_items < sm_count ? n_items : sm_count);
+  dim3 grid(n_items < sm_count ? n_items : sm_count);       // one persistent CTA per SM (192 KB of shared memory each)
   const CUtensorMap& q_lo = split3 ? q.lo : q.hi;
   const CUtensorMap& k_lo = split3 ? k.lo : k.hi;
   const CUtensorMap& v_lo = split3 ? vt.lo : vt.hi;
-#define MT3_AT_LAUNCH(S3, KSP, NC, MK)                                                                                           \
-  attention_tc_kernel<S3, KSP, NC, MK><<<grid, kAtThreads, kAtSmem, s>>>(q.hi, q_lo, k.hi, k_lo, vt.hi, v_lo, q_col0, k_col0, Tq, Tk, H, B, \
-                                                                         out_hi, out_lo, H * 64, TK, KS, part_o, part_ml, key_valid, n_valid)
-#define MT3_AT_FORMS(S3)                                \
-  if (KS > 1) MT3_AT_LAUNCH(S3, true, 2, 0);            \
-  else if (nchunk > 1) MT3_AT_LAUNCH(S3, false, 2, 0);  \
-  else MT3_AT_LAUNCH(S3, false, 1, 0);
+#define MT3_AT_LAUNCH(S3, KSP, NC, MK, PS)                                                                                            \
+  do {                                                                                                                                \
+    MT3_TRY((set_max_dynamic_smem<attention_tc_kernel<S3, KSP, NC, MK, PS>>(kAtSmem)));                                               \
+    attention_tc_kernel<S3, KSP, NC, MK, PS><<<grid, kAtThreads, kAtSmem, s>>>(q.hi, q_lo, k.hi, k_lo, vt.hi, v_lo, q_col0, k_col0, Tq, Tk, \
+                                                                               H, B, out_hi, out_lo, H * 64, TK, KS, part_o, part_ml,  \
+                                                                               key_valid, n_valid);                                    \
+  } while (0)
   // causal: items of two chunks always take the key-split instantiation, which writes the normalised output itself when
   // KS == 1 (Tk = 256); the single-pass two-chunk form spills with the mask's registers
-#define MT3_AT_CAUSAL_FORMS(S3)                         \
-  if (nchunk > 1) MT3_AT_LAUNCH(S3, true, 2, 1);        \
-  else MT3_AT_LAUNCH(S3, false, 1, 1);
-  if (split3 && causal) { MT3_AT_CAUSAL_FORMS(true) }
-  else if (split3) { MT3_AT_FORMS(true) }
-  else if (causal) { MT3_AT_CAUSAL_FORMS(false) }
-  else { MT3_AT_FORMS(false) }
-#undef MT3_AT_CAUSAL_FORMS
+#define MT3_AT_FORMS(S3, PS)                                                  \
+  if (causal && nchunk > 1) MT3_AT_LAUNCH(S3, true, 2, kAtMaskCausal, PS);    \
+  else if (causal) MT3_AT_LAUNCH(S3, false, 1, kAtMaskCausal, PS);            \
+  else if (KS > 1) MT3_AT_LAUNCH(S3, true, 2, kAtMaskNone, PS);               \
+  else if (nchunk > 1) MT3_AT_LAUNCH(S3, false, 2, kAtMaskNone, PS);          \
+  else MT3_AT_LAUNCH(S3, false, 1, kAtMaskNone, PS);
+  if (split3 && split_p) { MT3_AT_FORMS(true, true) }
+  else if (split3) { MT3_AT_FORMS(true, false) }
+  else { MT3_AT_FORMS(false, false) }
 #undef MT3_AT_FORMS
 #undef MT3_AT_LAUNCH
   MT3_LAUNCH_CHECK();
   if (KS > 1) {
     const long long items = (long long)B * Tq * H;
     if (causal)
-      attention_combine_causal_kernel<<<(unsigned)((items + 7) / 8), 256, 0, s>>>(part_o, part_ml, B, Tq, H, KS, TK, out_hi, out_lo);
+      attention_combine_kernel<true><<<(unsigned)((items + 7) / 8), 256, 0, s>>>(part_o, part_ml, B, Tq, H, KS, TK, out_hi, out_lo);
     else
-      enc_attention_combine_kernel<<<(unsigned)((items + 7) / 8), 256, 0, s>>>(part_o, part_ml, B, Tq, H, KS, out_hi, out_lo);
+      attention_combine_kernel<false><<<(unsigned)((items + 7) / 8), 256, 0, s>>>(part_o, part_ml, B, Tq, H, KS, TK, out_hi, out_lo);
     MT3_LAUNCH_CHECK();
   }
   return MT3_OK;

@@ -42,6 +42,24 @@ inline void count_launch(uint64_t n = 1) { g_launch_count.fetch_add(n, std::memo
     if (!(cond)) return ::mt3::fail(code, __VA_ARGS__);                                        \
   } while (0)
 
+#define MT3_TRY(expr)            \
+  do {                           \
+    int _r = (expr);             \
+    if (_r != MT3_OK) return _r; \
+  } while (0)
+
+// Raises Kernel's dynamic shared-memory limit to `bytes` before its first launch: once per kernel instantiation, as each
+// instantiation of this template has its own flag.
+template <auto Kernel>
+inline int set_max_dynamic_smem(int bytes) {
+  static bool done = false;
+  if (!done) {
+    MT3_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done = true;
+  }
+  return MT3_OK;
+}
+
 inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 

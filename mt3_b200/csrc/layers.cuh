@@ -1,5 +1,5 @@
 // Non-GEMM kernels of the MT3 encoder/decoder blocks (sm_90a): RMSNorm statistics,
-// attention (encoder, and the Tq = 1 decode form over the KV cache), token embedding,
+// full-sequence attention in fp32 (encoder, teacher-forced decoder), token embedding,
 // greedy argmax with EOS bookkeeping, vocabulary decode, weight re-layout.
 #pragma once
 
@@ -78,21 +78,20 @@ inline int launch_rmsnorm(const float* x, const float* x_lo, int ldx, int M, int
 }
 
 // ---------------------------------------------------------------------------------
-// Encoder self-attention, exact fp32 (layers.py:85-157): softmax(q k^T) v, no 1/sqrt(d)
-// scaling (layers.py:230-234), mask all ones (network.py:283-289).
-// qkv [B*T, 3*H*64] rows = (b,t), columns = [q | k | v] each (h, d).  out [B*T, H*64].
-// One CTA = 32 query rows of one (b, h); scores for all T keys live in shared memory.
+// Full-sequence attention, exact fp32 (layers.py:85-157): softmax(q k^T) v, no 1/sqrt(d)
+// scaling (layers.py:230-234); the encoder's mask is all ones (network.py:283-289).
+// One CTA = 32 query rows of one (b, h); scores for all Tk keys live in shared memory.
 // ---------------------------------------------------------------------------------
 constexpr int kHD = 64;   // head_dim the kernels are specialised for (gin/model.gin:54)
 
-// The work of one CTA, shared by the encoder kernel and the decoder's teacher-forced forms: queries of head h at columns
-// q_col0 + 64 h of q's rows [b Tq, (b + 1) Tq) (row pitch ldq), keys / values at k_col0 / v_col0 + 64 h of kv's rows
-// [b Tk, (b + 1) Tk) (row pitch ldkv).  CAUSAL: query i sees key j iff j <= i, j < n_valid and key_valid[b * n_valid + j]
-// > 0; key tiles past the CTA's last query are not read, and a row with no visible key writes 0.
+// Queries of head h at columns q_col0 + 64 h of q's rows [b Tq, (b + 1) Tq) (row pitch ldq), keys / values at k_col0 /
+// v_col0 + 64 h of kv's rows [b Tk, (b + 1) Tk) (row pitch ldkv).  CAUSAL: query i sees key j iff j <= i, j < n_valid and
+// key_valid[b * n_valid + j] > 0; key tiles past the CTA's last query are not read, and a row with no visible key writes 0.
 template <bool CAUSAL>
-__device__ __forceinline__ void attention_fp32_body(const float* __restrict__ q, int ldq, int q_col0, const float* __restrict__ kv, int ldkv,
-                                                    int k_col0, int v_col0, int Tq, int Tk, int H, float* __restrict__ out,
-                                                    float* __restrict__ out_lo, int ldo, const int* __restrict__ key_valid, int n_valid) {
+__global__ void __launch_bounds__(256)
+attention_fp32_kernel(const float* __restrict__ q, int ldq, int q_col0, const float* __restrict__ kv, int ldkv, int k_col0, int v_col0,
+                      int Tq, int Tk, int H, float* __restrict__ out, float* __restrict__ out_lo, int ldo,
+                      const int* __restrict__ key_valid, int n_valid) {
   extern __shared__ __align__(16) float sm[];
   constexpr int QT = 32, KT = 64;
   const int SP = Tk + 4;
@@ -212,54 +211,25 @@ __device__ __forceinline__ void attention_fp32_body(const float* __restrict__ q,
   store(q0 + tq + 16, o1);
 }
 
-__global__ void __launch_bounds__(256)
-enc_attention_kernel(const float* __restrict__ qkv, int ld, int T, int H, float* __restrict__ out,
-                     float* __restrict__ out_lo, int ldo) {
-  attention_fp32_body<false>(qkv, ld, 0, qkv, ld, H * kHD, 2 * H * kHD, T, T, H, out, out_lo, ldo, nullptr, 0);
-}
+// Shared memory of attention_fp32_kernel: sQ, sS and sT.  The row of scores over all Tk keys (sS) bounds Tk.
+constexpr size_t kAttFp32MaxSmem = 200 * 1024;
+inline size_t attention_fp32_smem(int Tk) { return (size_t)(32 * kHD + 32 * (Tk + 4) + 64 * 68) * sizeof(float); }
 
-template <bool CAUSAL>
-__global__ void __launch_bounds__(256)
-attention_fp32_kernel(const float* __restrict__ q, int ldq, int q_col0, const float* __restrict__ kv, int ldkv, int k_col0, int v_col0,
-                      int Tq, int Tk, int H, float* __restrict__ out, float* __restrict__ out_lo, int ldo,
-                      const int* __restrict__ key_valid, int n_valid) {
-  attention_fp32_body<CAUSAL>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, key_valid, n_valid);
-}
-
-// sQ, sS and sT of enc_attention_kernel; the scores of all T keys bound T.
-constexpr size_t kEncAttMaxSmem = 200 * 1024;
-inline size_t enc_attention_smem(int T) { return (size_t)(32 * kHD + 32 * (T + 4) + 64 * 68) * sizeof(float); }
-
-inline int launch_enc_attention(const float* qkv, int ld, int T, int H, int B, float* out, float* out_lo, int ldo, cudaStream_t s) {
-  const size_t smem = enc_attention_smem(T);
-  MT3_REQUIRE(smem <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "encoder attention: T=%d too long", T);
-  static bool attr_done = false;
-  if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(enc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
-    attr_done = true;
-  }
-  enc_attention_kernel<<<dim3(cdiv(T, 32), H, B), 256, smem, s>>>(qkv, ld, T, H, out, out_lo, ldo);
-  MT3_LAUNCH_CHECK();
-  return MT3_OK;
-}
-
-// The decoder's teacher-forced forms (attention_fp32_body): causal self-attention over the [B*Tq, 3Q] qkv rows with per-key
-// validity (key_valid != null), or cross-attention of q [B*Tq, ldq] over kv [B*Tk, ldkv].  out [B*Tq, H*64].
+// Encoder self-attention over the [B*T, 3Q] qkv rows (q = kv = qkv, k_col0 = Q, v_col0 = 2Q); the teacher-forced decoder's
+// causal self-attention with per-key validity (key_valid != null), and its cross-attention of q [B*Tq, ldq] over
+// kv [B*Tk, ldkv].  out [B*Tq, H*64].
 inline int launch_attention_fp32(const float* q, int ldq, int q_col0, const float* kv, int ldkv, int k_col0, int v_col0, int Tq, int Tk, int H,
                                  int B, float* out, float* out_lo, int ldo, const int* key_valid, int n_valid, cudaStream_t s) {
-  const size_t smem = enc_attention_smem(Tk);
-  MT3_REQUIRE(smem <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "fp32 attention: Tk=%d too long", Tk);
-  static bool attr_done = false;
-  if (!attr_done) {
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
-    MT3_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEncAttMaxSmem));
-    attr_done = true;
-  }
+  const size_t smem = attention_fp32_smem(Tk);
+  MT3_REQUIRE(smem <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED, "fp32 attention: Tk=%d too long", Tk);
   const dim3 grid(cdiv(Tq, 32), H, B);
-  if (key_valid)
+  if (key_valid) {
+    MT3_TRY(set_max_dynamic_smem<attention_fp32_kernel<true>>((int)kAttFp32MaxSmem));
     attention_fp32_kernel<true><<<grid, 256, smem, s>>>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, key_valid, n_valid);
-  else
+  } else {
+    MT3_TRY(set_max_dynamic_smem<attention_fp32_kernel<false>>((int)kAttFp32MaxSmem));
     attention_fp32_kernel<false><<<grid, 256, smem, s>>>(q, ldq, q_col0, kv, ldkv, k_col0, v_col0, Tq, Tk, H, out, out_lo, ldo, nullptr, 0);
+  }
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }

@@ -133,7 +133,6 @@ struct Model {
   float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
   int dcounters_n = 0;
   int* dcounters = nullptr;
-  int sm_count = 132;
   bool have_cross = false;
   int host_pos = 0;               // host mirror of the device position (cache overflow guard)
 
@@ -188,11 +187,6 @@ static int prep_copy(cudaStream_t s, const float* src, int K, int N, const float
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
-#define MT3_TRY(expr)            \
-  do {                           \
-    int _r = (expr);             \
-    if (_r != MT3_OK) return _r; \
-  } while (0)
 
 static int prep_tc_weight(Model* m, cudaStream_t s, const float* w, int K, int N, float*& cursor, TcW* out) {
   out->K = K; out->N = N;
@@ -235,79 +229,98 @@ static int enc_gemm(const Model* m, const Act& A, const float* w, const TcW& tw,
   return launch_sgemm(a, s);
 }
 
-// x [B*T, K], owned by the caller, as the A operand of an encoder-side GEMM; in TF32X3 mode it is split into `pair` first.
-static int enc_input(const Model* m, const float* x, int K, const Act& pair, Act* out, cudaStream_t s) {
-  const int M = m->B * m->T;
+// an activation [rows, cols] (lo null unless TF32X3); on the wgmma path also its TMA operand
+static int make_act(const Model* m, float* hi, float* lo, int64_t rows, int cols, Act* a, uint32_t box_rows = 128) {
+  a->hi = hi; a->lo = lo;
+  return m->tc ? make_operand(&a->op, hi, lo, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, box_rows) : MT3_OK;
+}
+
+// x [M, K], owned by the caller, as the A operand of an encoder-side GEMM; in TF32X3 mode it is split into `pair` first.
+static int enc_input(const Model* m, const float* x, int64_t M, int K, const Act& pair, Act* out, cudaStream_t s) {
   if (m->split3) {
-    const long long n4 = (long long)M * K / 4;
+    const long long n4 = M * K / 4;
     split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(x, pair.hi, pair.lo, n4);
     MT3_LAUNCH_CHECK();
     *out = pair;
     return MT3_OK;
   }
-  out->hi = const_cast<float*>(x);
-  return m->tc ? make_operand(&out->op, x, nullptr, M, K, K) : MT3_OK;
+  return make_act(m, const_cast<float*>(x), nullptr, M, K, out);
 }
 
-static bool enc_tc_attention(const Model* m) { return m->tc && m->tc_attn_ok && enc_attention_tc_supported(m->T); }
-
-// Encoder layer steps (network.py:44-85).  RMSNorm statistic of the residual stream h, applied as the next GEMM's row scale
-static int enc_rstd(Model* m, cudaStream_t s) {
-  return launch_row_rstd(m->a_h.hi, m->a_h.lo, m->D, m->B * m->T, m->D, 1e-6f, m->rstd, s);
+// Attention on the wgmma kernel: the mode asks for it and the kernel takes the shape.
+static bool tc_attention(const Model* m, int Tq, int Tk, bool causal) {
+  return m->tc && m->tc_attn_ok && attention_tc_supported(Tq, Tk, causal);
 }
-// QKV projection.  When the wgmma attention consumes qkv it goes out as a tf32 hi/lo pair (TF32X3), and the V third also
-// transposed per head: the K-major operand of P.V.
-static int enc_layer_qkv(Model* m, int l, cudaStream_t s) {
+
+// The layer steps of a full sequence, shared by the encoder (network.py:44-85) and the teacher-forced decoder pass
+// (:88-155): M rows of the residual stream h.  RMSNorm statistic of h, applied as the next GEMM's row scale
+static int seq_rstd(const Model* m, const Act& h, int M, float* rstd, cudaStream_t s) {
+  return launch_row_rstd(h.hi, h.lo, m->D, M, m->D, 1e-6f, rstd, s);
+}
+// QKV projection into qkv [M, 3Q].  vt: the wgmma self-attention's operands, which need qkv as a tf32 hi/lo pair (TF32X3)
+// and the V third also transposed per head into vt [B*H*64, T] (T rows per sequence): the K-major operand of P.V
+static int seq_qkv(const Model* m, const Act& h, int M, const float* rstd, const float* w, const TcW& tw, const Act& qkv, const Act* vt,
+                   int T, cudaStream_t s) {
   const int Q = m->Q;
-  const bool tc_attn = enc_tc_attention(m);
-  TcGemmArgs a = gemm_epi(m->B * m->T, 3 * Q, m->D, m->a_qkv.hi, tc_attn ? m->a_qkv.lo : nullptr, 3 * Q);
-  a.row_scale = m->rstd;
-  if (tc_attn) {
-    a.VT_hi = m->a_vt.hi; a.VT_lo = m->a_vt.lo; a.vt_col0 = 2 * Q; a.vt_T = m->T; a.vt_H = m->H;
+  TcGemmArgs a = gemm_epi(M, 3 * Q, m->D, qkv.hi, vt ? qkv.lo : nullptr, 3 * Q);
+  a.row_scale = rstd;
+  if (vt) {
+    a.VT_hi = vt->hi; a.VT_lo = vt->lo; a.vt_col0 = 2 * Q; a.vt_T = T; a.vt_H = m->H;
   }
-  return enc_gemm(m, m->a_h, m->enc[l].wqkv, m->enc[l].t_wqkv, a, s);
+  return enc_gemm(m, h, w, tw, a, s);
 }
-static int enc_layer_attn(Model* m, cudaStream_t s) {
-  if (enc_tc_attention(m))
-    return launch_enc_attention_tc(m->a_qkv.op, m->a_vt.op, m->B, m->T, m->H, m->a_ao.hi, m->a_ao.lo, m->split3, s, m->att_scratch);
-  return launch_enc_attention(m->a_qkv.hi, 3 * m->Q, m->T, m->H, m->B, m->a_ao.hi, m->a_ao.lo, m->Q, s);
+// Self-attention of B sequences of T rows from qkv into ao: on the wgmma kernel when vt (seq_qkv) is given, else exact fp32.
+// key_valid [B, n_valid]: causal with per-key validity (make_decoder_mask); null: every key visible.  split_p: P . V in
+// 3xTF32 too (TF32X3; see attention_tc_kernel's PSPLIT).
+static int seq_self_attention(const Model* m, const Act& qkv, const Act* vt, int B, int T, const int* key_valid, int n_valid, bool split_p,
+                              const Act& ao, float* scratch, cudaStream_t s) {
+  const int Q = m->Q;
+  if (vt)
+    return launch_attention_tc(qkv.op, 0, T, qkv.op, Q, T, vt->op, B, m->H, ao.hi, ao.lo, m->split3, split_p, key_valid != nullptr,
+                               key_valid, n_valid, s, scratch);
+  return launch_attention_fp32(qkv.hi, 3 * Q, 0, qkv.hi, 3 * Q, Q, 2 * Q, T, T, m->H, B, ao.hi, ao.lo, Q, key_valid, n_valid, s);
 }
-// h += A . W: the attention out-projection (A = ao) and the MLP out-projection (A = g)
-static int enc_layer_residual(Model* m, const Act& A, int K, const float* w, const TcW& tw, cudaStream_t s) {
+// h += A . W: the attention out-projections (A = attention output) and the MLP out-projection (A = g)
+static int seq_residual(const Model* m, const Act& h, int M, const Act& A, int K, const float* w, const TcW& tw, cudaStream_t s) {
   const int D = m->D;
-  TcGemmArgs a = gemm_epi(m->B * m->T, D, K, m->a_h.hi, m->a_h.lo, D);
-  a.epi = EPI_RESIDUAL; a.R_hi = m->a_h.hi; a.R_lo = m->a_h.lo; a.ldr = D;
+  TcGemmArgs a = gemm_epi(M, D, K, h.hi, h.lo, D);
+  a.epi = EPI_RESIDUAL; a.R_hi = h.hi; a.R_lo = h.lo; a.ldr = D;
   return enc_gemm(m, A, w, tw, a, s);
 }
-static int enc_layer_mlp_in(Model* m, int l, cudaStream_t s) {
+// gated-GELU MLP-in into g [M, F]
+static int seq_mlp_in(const Model* m, const Act& h, int M, const float* rstd, const float* w, const TcW& tw, const Act& g, cudaStream_t s) {
   const int F = m->F;
-  TcGemmArgs a = gemm_epi(m->B * m->T, 2 * F, m->D, m->a_g.hi, m->a_g.lo, F);
-  a.row_scale = m->rstd; a.epi = EPI_GATED_GELU;
-  return enc_gemm(m, m->a_h, m->enc[l].wi, m->enc[l].t_wi, a, s);
+  TcGemmArgs a = gemm_epi(M, 2 * F, m->D, g.hi, g.lo, F);
+  a.row_scale = rstd; a.epi = EPI_GATED_GELU;
+  return enc_gemm(m, h, w, tw, a, s);
 }
+
+// the encoder's V^T target where its attention runs on the wgmma kernel, else null
+static const Act* enc_vt(const Model* m) { return tc_attention(m, m->T, m->T, false) ? &m->a_vt : nullptr; }
 
 // Encoder (network.py:158-193): input projection + PE, the layers, and the closing RMSNorm into `encoded`.
 static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s) {
   const int M = m->B * m->T, D = m->D, depth = m->cfg.input_depth;
   // the exact-fp32 attention kernel's limit, in every mode
-  MT3_REQUIRE(enc_attention_smem(m->T) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel",
+  MT3_REQUIRE(attention_fp32_smem(m->T) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel",
               m->T);
   Act ax;
-  MT3_TRY(enc_input(m, x, depth, m->a_x, &ax, s));
+  MT3_TRY(enc_input(m, x, M, depth, m->a_x, &ax, s));
   {
     TcGemmArgs a = gemm_epi(M, D, depth, m->a_h.hi, m->a_h.lo, D);
     a.epi = EPI_ADD_PE; a.pe = m->pe; a.pe_T = m->T; a.pe_ld = D;
     MT3_TRY(enc_gemm(m, ax, m->w_in, m->t_w_in, a, s));
   }
+  const Act* vt = enc_vt(m);
   for (int l = 0; l < m->Le; ++l) {
     const EncLayer& w = m->enc[l];
-    MT3_TRY(enc_rstd(m, s));
-    MT3_TRY(enc_layer_qkv(m, l, s));
-    MT3_TRY(enc_layer_attn(m, s));
-    MT3_TRY(enc_layer_residual(m, m->a_ao, m->Q, w.wo, w.t_wo, s));
-    MT3_TRY(enc_rstd(m, s));
-    MT3_TRY(enc_layer_mlp_in(m, l, s));
-    MT3_TRY(enc_layer_residual(m, m->a_g, m->F, w.wo2, w.t_wo2, s));
+    MT3_TRY(seq_rstd(m, m->a_h, M, m->rstd, s));
+    MT3_TRY(seq_qkv(m, m->a_h, M, m->rstd, w.wqkv, w.t_wqkv, m->a_qkv, vt, m->T, s));
+    MT3_TRY(seq_self_attention(m, m->a_qkv, vt, m->B, m->T, nullptr, 0, false, m->a_ao, m->att_scratch, s));
+    MT3_TRY(seq_residual(m, m->a_h, M, m->a_ao, m->Q, w.wo, w.t_wo, s));
+    MT3_TRY(seq_rstd(m, m->a_h, M, m->rstd, s));
+    MT3_TRY(seq_mlp_in(m, m->a_h, M, m->rstd, w.wi, w.t_wi, m->a_g, s));
+    MT3_TRY(seq_residual(m, m->a_h, M, m->a_g, m->F, w.wo2, w.t_wo2, s));
   }
   return launch_rmsnorm(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->enc_norm_g, encoded, D, s);
 }
@@ -316,7 +329,7 @@ static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s)
 static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
   const int M = m->B * m->T, D = m->D, Q = m->Q;
   Act ae;
-  MT3_TRY(enc_input(m, encoded, D, m->a_enc, &ae, s));
+  MT3_TRY(enc_input(m, encoded, M, D, m->a_enc, &ae, s));
   for (int l = 0; l < m->Ld; ++l) {
     TcGemmArgs a = gemm_epi(M, 2 * Q, D, nullptr, nullptr, 2 * Q);
     a.n_split = 0; a.C1 = kv_layer(m, m->ckv, l, m->T); a.kv_fmt = m->kv_fmt; a.hm_rows_per_b = m->T; a.hm_cap = m->T; a.hm_H = m->H;
@@ -574,8 +587,6 @@ static int ensure_graph(Model* m, int mode, int nsteps = 1) {
 constexpr int kTfLogitRows = 8192;   // logits rows per chunk of the logits GEMM + score kernel (50 MB at V = 1536)
 
 static int tf_pad(int L) { return cdiv(L, kAtQ) * kAtQ; }
-static bool tf_self_tc(const Model* m) { return m->tc && m->tc_attn_ok; }
-static bool tf_cross_tc(const Model* m, int T) { return m->tc && m->tc_attn_ok && enc_attention_tc_supported(T); }
 
 struct TfLayout {
   int64_t y, y_lo, rstd, qkv, qkv_lo, vt, vt_lo, ao, ao_lo, qc, qc_lo, enc, enc_lo, ckv, ckv_lo, cvt, cvt_lo, g, g_lo, scratch, logits, total;
@@ -586,7 +597,7 @@ static TfLayout tf_layout(const Model* m, int B, int T, int L) {
   auto take = [&](int64_t bytes) { int64_t r = off; off += align_up(bytes, 256); return r; };
   const int Lp = tf_pad(L);
   const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T, D = m->D, Q = m->Q, F = m->F, V = m->V;
-  const bool s3 = m->split3, tcs = tf_self_tc(m), tcc = tf_cross_tc(m, T);
+  const bool s3 = m->split3, tcs = tc_attention(m, Lp, Lp, true), tcc = tc_attention(m, Lp, T, false);
   w.y = take(M * D * 4);                          // residual stream (hi/lo in TF32X3)
   w.y_lo = take(s3 ? M * D * 4 : 0);
   w.rstd = take(M * 4);
@@ -650,90 +661,62 @@ static int ensure_tf_weights(Model* m, cudaStream_t s) {
   return MT3_OK;
 }
 
-// an activation [rows, cols] of the pass (lo null unless TF32X3); on the wgmma path also its TMA operand
-static int tf_act(const Model* m, float* hi, float* lo, int64_t rows, int cols, Act* a, uint32_t box_rows = 128) {
-  a->hi = hi; a->lo = lo;
-  return m->tc ? make_operand(&a->op, hi, lo, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, box_rows) : MT3_OK;
-}
-
 static int teacher_forced_impl(Model* m, const float* encoded, int B, int T, const int* tok_in, const int* tgt, const int* wts, int L,
                                float* logits, float* scores, char* ws, cudaStream_t s) {
   const int Lp = tf_pad(L), D = m->D, Q = m->Q, F = m->F, V = m->V, H = m->H;
-  const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T;
-  const bool s3 = m->split3, tcs = tf_self_tc(m), tcc = tf_cross_tc(m, T);
+  const int M = B * Lp, Me = B * T;
+  const bool s3 = m->split3, tcs = tc_attention(m, Lp, Lp, true), tcc = tc_attention(m, Lp, T, false);
   const TfLayout w = tf_layout(m, B, T, L);
   auto P = [&](int64_t off, bool on = true) { return on ? (float*)(ws + off) : nullptr; };
-  Act y, qkv, vt, ao, qc, enc, ckv, cvt, g;
-  MT3_TRY(tf_act(m, P(w.y), P(w.y_lo, s3), M, D, &y));
-  MT3_TRY(tf_act(m, P(w.ao), P(w.ao_lo, s3), M, Q, &ao));
-  MT3_TRY(tf_act(m, P(w.g), P(w.g_lo, s3), M, F, &g));
-  MT3_TRY(tf_act(m, P(w.qkv), P(w.qkv_lo, s3 && tcs), M, 3 * Q, &qkv));
-  MT3_TRY(tf_act(m, P(w.qc), P(w.qc_lo, s3 && tcc), M, Q, &qc));
-  MT3_TRY(tf_act(m, P(w.ckv), P(w.ckv_lo, s3 && tcc), Me, 2 * Q, &ckv));
-  if (tcs) MT3_TRY(tf_act(m, P(w.vt), P(w.vt_lo, s3), (int64_t)B * H * 64, Lp, &vt, 64));
-  if (tcc) MT3_TRY(tf_act(m, P(w.cvt), P(w.cvt_lo, s3), (int64_t)B * H * 64, T, &cvt, 64));
-  if (s3) {
-    const long long n4 = Me * D / 4;
-    split_pair_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(encoded, P(w.enc), P(w.enc_lo), n4);
-    MT3_LAUNCH_CHECK();
-    MT3_TRY(tf_act(m, P(w.enc), P(w.enc_lo), Me, D, &enc));
-  } else {
-    MT3_TRY(tf_act(m, const_cast<float*>(encoded), nullptr, Me, D, &enc));
-  }
+  Act y, qkv, vt, ao, qc, enc_pair, enc, ckv, cvt, g;
+  MT3_TRY(make_act(m, P(w.y), P(w.y_lo, s3), M, D, &y));
+  MT3_TRY(make_act(m, P(w.ao), P(w.ao_lo, s3), M, Q, &ao));
+  MT3_TRY(make_act(m, P(w.g), P(w.g_lo, s3), M, F, &g));
+  MT3_TRY(make_act(m, P(w.qkv), P(w.qkv_lo, s3 && tcs), M, 3 * Q, &qkv));
+  MT3_TRY(make_act(m, P(w.qc), P(w.qc_lo, s3 && tcc), M, Q, &qc));
+  MT3_TRY(make_act(m, P(w.ckv), P(w.ckv_lo, s3 && tcc), Me, 2 * Q, &ckv));
+  if (tcs) MT3_TRY(make_act(m, P(w.vt), P(w.vt_lo, s3), (int64_t)B * H * 64, Lp, &vt, 64));
+  if (tcc) MT3_TRY(make_act(m, P(w.cvt), P(w.cvt_lo, s3), (int64_t)B * H * 64, T, &cvt, 64));
+  if (s3) MT3_TRY(make_act(m, P(w.enc), P(w.enc_lo), Me, D, &enc_pair));
+  MT3_TRY(enc_input(m, encoded, Me, D, enc_pair, &enc, s));
   float* rstd = P(w.rstd);
   float* scratch = P(w.scratch, w.logits > w.scratch);
-  auto norm = [&]() { return launch_row_rstd(y.hi, y.lo, D, (int)M, D, 1e-6f, rstd, s); };
-  auto residual = [&](const Act& A, int K, const float* wt, const TcW& tw) {     // y += A . W
-    TcGemmArgs a = gemm_epi((int)M, D, K, y.hi, y.lo, D);
-    a.epi = EPI_RESIDUAL; a.R_hi = y.hi; a.R_lo = y.lo; a.ldr = D;
-    return enc_gemm(m, A, wt, tw, a, s);
-  };
 
   MT3_TRY(launch_embed_seq(tok_in, B, L, Lp, m->emb, D, V, m->pe, y.hi, y.lo, s));
   for (int l = 0; l < m->Ld; ++l) {
     const DecLayer& dl = m->dec[l];
     // self-attention: RMSNorm folded into the QKV projection's row scale; mask make_decoder_mask(targets)
-    MT3_TRY(norm());
-    {
-      TcGemmArgs a = gemm_epi((int)M, 3 * Q, D, qkv.hi, qkv.lo, 3 * Q);
-      a.row_scale = rstd;
-      if (tcs) { a.VT_hi = vt.hi; a.VT_lo = vt.lo; a.vt_col0 = 2 * Q; a.vt_T = Lp; a.vt_H = H; }
-      MT3_TRY(enc_gemm(m, y, dl.wqkv, dl.t_wqkv, a, s));
-    }
-    if (tcs) MT3_TRY(launch_attention_tc(qkv.op, 0, Lp, qkv.op, Q, Lp, vt.op, B, H, ao.hi, ao.lo, s3, true, tgt, L, s, scratch));
-    else MT3_TRY(launch_attention_fp32(qkv.hi, 3 * Q, 0, qkv.hi, 3 * Q, Q, 2 * Q, Lp, Lp, H, B, ao.hi, ao.lo, Q, tgt, L, s));
-    MT3_TRY(residual(ao, Q, dl.wo, dl.t_wo));
+    MT3_TRY(seq_rstd(m, y, M, rstd, s));
+    MT3_TRY(seq_qkv(m, y, M, rstd, dl.wqkv, dl.t_wqkv, qkv, tcs ? &vt : nullptr, Lp, s));
+    MT3_TRY(seq_self_attention(m, qkv, tcs ? &vt : nullptr, B, Lp, tgt, L, true, ao, scratch, s));
+    MT3_TRY(seq_residual(m, y, M, ao, Q, dl.wo, dl.t_wo, s));
     // cross-attention over all T encoder positions; K/V projected from `encoded` for this layer
-    MT3_TRY(norm());
+    MT3_TRY(seq_rstd(m, y, M, rstd, s));
     {
-      TcGemmArgs a = gemm_epi((int)M, Q, D, qc.hi, qc.lo, Q);
+      TcGemmArgs a = gemm_epi(M, Q, D, qc.hi, qc.lo, Q);
       a.row_scale = rstd;
       MT3_TRY(enc_gemm(m, y, dl.wq_c, dl.t_wq_c, a, s));
     }
     {
-      TcGemmArgs a = gemm_epi((int)Me, 2 * Q, D, ckv.hi, ckv.lo, 2 * Q);
+      TcGemmArgs a = gemm_epi(Me, 2 * Q, D, ckv.hi, ckv.lo, 2 * Q);
       if (tcc) { a.VT_hi = cvt.hi; a.VT_lo = cvt.lo; a.vt_col0 = Q; a.vt_T = T; a.vt_H = H; }
       MT3_TRY(enc_gemm(m, enc, dl.wkv_c, dl.t_wkv_c, a, s));
     }
-    if (tcc) MT3_TRY(launch_attention_tc(qc.op, 0, Lp, ckv.op, 0, T, cvt.op, B, H, ao.hi, ao.lo, s3, false, nullptr, 0, s, scratch));
+    if (tcc) MT3_TRY(launch_attention_tc(qc.op, 0, Lp, ckv.op, 0, T, cvt.op, B, H, ao.hi, ao.lo, s3, true, false, nullptr, 0, s, scratch));
     else MT3_TRY(launch_attention_fp32(qc.hi, Q, 0, ckv.hi, 2 * Q, 0, Q, Lp, T, H, B, ao.hi, ao.lo, Q, nullptr, 0, s));
-    MT3_TRY(residual(ao, Q, dl.wo_c, dl.t_wo_c));
+    MT3_TRY(seq_residual(m, y, M, ao, Q, dl.wo_c, dl.t_wo_c, s));
     // gated-GELU MLP
-    MT3_TRY(norm());
-    {
-      TcGemmArgs a = gemm_epi((int)M, 2 * F, D, g.hi, g.lo, F);
-      a.row_scale = rstd; a.epi = EPI_GATED_GELU;
-      MT3_TRY(enc_gemm(m, y, dl.wi, dl.t_wi, a, s));
-    }
-    MT3_TRY(residual(g, F, dl.wo2, dl.t_wo2));
+    MT3_TRY(seq_rstd(m, y, M, rstd, s));
+    MT3_TRY(seq_mlp_in(m, y, M, rstd, dl.wi, dl.t_wi, g, s));
+    MT3_TRY(seq_residual(m, y, M, g, F, dl.wo2, dl.t_wo2, s));
   }
   // decoder_norm (folded into w_logits) + logits_dense, then the scores, in chunks of rows
-  MT3_TRY(norm());
+  MT3_TRY(seq_rstd(m, y, M, rstd, s));
   float* chunk = P(w.logits);
   for (int64_t r0 = 0; r0 < M; r0 += kTfLogitRows) {
     const int n = (int)std::min((int64_t)kTfLogitRows, M - r0);
     Act ys;
-    MT3_TRY(tf_act(m, y.hi + r0 * D, y.lo ? y.lo + r0 * D : nullptr, n, D, &ys));
+    MT3_TRY(make_act(m, y.hi + r0 * D, y.lo ? y.lo + r0 * D : nullptr, n, D, &ys));
     TcGemmArgs a = gemm_epi(n, V, D, chunk, nullptr, V);
     a.row_scale = rstd + r0;
     MT3_TRY(enc_gemm(m, ys, m->w_logits, m->t_w_logits, a, s));
@@ -874,11 +857,6 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
     if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: PE upload -> %s", cudaGetErrorString(e));
   }
   {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
-      m->sm_count = sms;
-  }
-  {
     const char* e_pdl = getenv("MT3_PDL");
     m->pdl_attn = !(e_pdl && e_pdl[0] == '0');
     const char* e_attn = getenv("MT3_TC_ATTENTION");
@@ -985,7 +963,7 @@ WsLayout ws_layout(const Model* m, int B, int T) {
   w.state = take(64);
   w.dpartial = take((int64_t)16 * cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * kDecTileFloats * 4);   // up to 16 K chunks
   w.dcounters = take((int64_t)cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * 4);
-  w.att_scratch = take(m->tc ? enc_attention_tc_scratch_floats(B, T, m->H) * 4 : 0);
+  w.att_scratch = take(m->tc ? attention_tc_scratch_floats(B, T, T, m->H, false) * 4 : 0);
   w.beam_f = take((int64_t)B * 2 * 4);
   w.beam_i = take((int64_t)B * 4);
   w.total = off;
@@ -1018,30 +996,22 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
   m->finished = (int*)(b + w.finished); m->tokens = (int*)(b + w.tokens); m->state = (int*)(b + w.state);
   m->dpartial = (float*)(b + w.dpartial); m->dcounters = (int*)(b + w.dcounters);
   m->beam_f = (float*)(b + w.beam_f); m->beam_i = (int*)(b + w.beam_i);
-  m->att_scratch = (m->tc && enc_attention_tc_scratch_floats(batch, input_length, m->H) > 0) ? (float*)(b + w.att_scratch) : nullptr;
+  const bool key_split = m->tc && attention_tc_scratch_floats(batch, input_length, input_length, m->H, false) > 0;
+  m->att_scratch = key_split ? (float*)(b + w.att_scratch) : nullptr;
   m->dcounters_n = cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN);
   m->have_cross = false;
-  const bool s3 = m->split3;
-  m->a_h.hi = m->h; m->a_h.lo = s3 ? (float*)(b + w.h_lo) : nullptr;
-  m->a_ao.hi = m->ao; m->a_ao.lo = s3 ? (float*)(b + w.ao_lo) : nullptr;
-  m->a_g.hi = m->g; m->a_g.lo = s3 ? (float*)(b + w.g_lo) : nullptr;
-  m->a_qkv.hi = m->qkv; m->a_qkv.lo = s3 ? (float*)(b + w.qkv_lo) : nullptr;
-  if (m->tc) {
-    const int64_t M = (int64_t)batch * input_length;
-    m->a_x.hi = s3 ? (float*)(b + w.x_hi) : nullptr; m->a_x.lo = s3 ? (float*)(b + w.x_lo) : nullptr;
-    m->a_enc.hi = s3 ? (float*)(b + w.enc_hi) : nullptr; m->a_enc.lo = s3 ? (float*)(b + w.enc_lo) : nullptr;
-    if (s3) {
-      MT3_TRY(make_operand(&m->a_x.op, m->a_x.hi, m->a_x.lo, M, m->cfg.input_depth, m->cfg.input_depth));
-      MT3_TRY(make_operand(&m->a_enc.op, m->a_enc.hi, m->a_enc.lo, M, m->D, m->D));
-    }
-    MT3_TRY(make_operand(&m->a_h.op, m->a_h.hi, m->a_h.lo, M, m->D, m->D));
-    MT3_TRY(make_operand(&m->a_ao.op, m->a_ao.hi, m->a_ao.lo, M, m->Q, m->Q));
-    MT3_TRY(make_operand(&m->a_g.op, m->a_g.hi, m->a_g.lo, M, m->F, m->F));
-    MT3_TRY(make_operand(&m->a_qkv.op, m->a_qkv.hi, m->a_qkv.lo, M, 3 * m->Q, 3 * m->Q));
-    m->a_vt.hi = (float*)(b + w.vt_hi); m->a_vt.lo = s3 ? (float*)(b + w.vt_lo) : nullptr;
-    if (input_length % 4 == 0)   // TMA row pitch must be a multiple of 16 bytes; otherwise the SIMT attention kernel runs
-      MT3_TRY(make_operand(&m->a_vt.op, m->a_vt.hi, m->a_vt.lo, (uint64_t)batch * m->H * 64, input_length, input_length, 64));
+  const int64_t M = (int64_t)batch * input_length;
+  auto lo = [&](int64_t off) { return m->split3 ? (float*)(b + off) : nullptr; };
+  MT3_TRY(make_act(m, m->h, lo(w.h_lo), M, m->D, &m->a_h));
+  MT3_TRY(make_act(m, m->ao, lo(w.ao_lo), M, m->Q, &m->a_ao));
+  MT3_TRY(make_act(m, m->g, lo(w.g_lo), M, m->F, &m->a_g));
+  MT3_TRY(make_act(m, m->qkv, lo(w.qkv_lo), M, 3 * m->Q, &m->a_qkv));
+  if (m->split3) {
+    MT3_TRY(make_act(m, (float*)(b + w.x_hi), lo(w.x_lo), M, m->cfg.input_depth, &m->a_x));
+    MT3_TRY(make_act(m, (float*)(b + w.enc_hi), lo(w.enc_lo), M, m->D, &m->a_enc));
   }
+  if (m->tc && input_length % 4 == 0)   // TMA row pitch must be a multiple of 16 bytes; otherwise the SIMT attention kernel runs
+    MT3_TRY(make_act(m, (float*)(b + w.vt_hi), lo(w.vt_lo), (int64_t)batch * m->H * 64, input_length, &m->a_vt, 64));
   return MT3_OK;
 }
 
@@ -1165,9 +1135,10 @@ extern "C" int mt3_decode_teacher_forced(mt3_model* h, const float* encoded, int
   MT3_REQUIRE(workspace_bytes >= w.total, MT3_ERR_WORKSPACE, "workspace has %lld bytes, %lld needed", (long long)workspace_bytes,
               (long long)w.total);
   // the exact-fp32 attention kernel's limit where it runs, and the wgmma GEMM's N tiling of the logits projection
-  MT3_REQUIRE(tf_self_tc(m) || enc_attention_smem(tf_pad(target_length)) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED,
+  const int Lp = tf_pad(target_length);
+  MT3_REQUIRE(tc_attention(m, Lp, Lp, true) || attention_fp32_smem(Lp) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED,
               "mt3_decode_teacher_forced: target_length %d too long for the exact-fp32 attention kernel", target_length);
-  MT3_REQUIRE(tf_cross_tc(m, input_length) || enc_attention_smem(input_length) <= kEncAttMaxSmem, MT3_ERR_UNSUPPORTED,
+  MT3_REQUIRE(tc_attention(m, Lp, input_length, false) || attention_fp32_smem(input_length) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED,
               "mt3_decode_teacher_forced: input_length %d too long for the exact-fp32 attention kernel", input_length);
   MT3_REQUIRE(!m->tc || m->V % 32 == 0, MT3_ERR_UNSUPPORTED, "mt3_decode_teacher_forced: the wgmma logits GEMM needs vocab %% 32 == 0");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1282,11 +1253,12 @@ extern "C" int mt3_debug_launch(mt3_model* h, int32_t kind, int32_t pos, int32_t
         break;
       }
       case MT3_K_ENC_QKV_GEMM: {
-        MT3_TRY(enc_layer_qkv(m, it % std::max(1, m->Le), s));
+        const EncLayer& w = m->enc[it % std::max(1, m->Le)];
+        MT3_TRY(seq_qkv(m, m->a_h, m->B * T, m->rstd, w.wqkv, w.t_wqkv, m->a_qkv, enc_vt(m), T, s));
         break;
       }
       case MT3_K_ENC_ATTN: {
-        MT3_TRY(enc_layer_attn(m, s));
+        MT3_TRY(seq_self_attention(m, m->a_qkv, enc_vt(m), m->B, T, nullptr, 0, false, m->a_ao, m->att_scratch, s));
         break;
       }
       default:

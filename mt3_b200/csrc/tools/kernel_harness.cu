@@ -80,30 +80,31 @@ KH_API int kh_tc_gemm(const float* a_hi, const float* a_lo, int lda, const float
 
 KH_API int kh_sgemm(const GemmArgs* a) { return launch_sgemm(*a, 0); }
 
-// qkv [B*T, 3*H*64] (hi, lo), vt [B*H*64, T] (hi, lo; keys in vt_key_slot() order), out [B*T, H*64]
+// The encoder's form of the attention kernels.  qkv [B*T, 3*H*64] (hi, lo), vt [B*H*64, T] (hi, lo; keys in vt_key_slot()
+// order), out [B*T, H*64]
 KH_API int kh_enc_attention_tc(const float* qkv_hi, const float* qkv_lo, const float* vt_hi, const float* vt_lo, int B, int T, int H,
                         float* out_hi, float* out_lo, int split3, float* scratch) {
-  MT3_REQUIRE(enc_attention_tc_supported(T), MT3_ERR_UNSUPPORTED, "tc attention: T=%d is not supported", T);
+  MT3_REQUIRE(attention_tc_supported(T, T, false), MT3_ERR_UNSUPPORTED, "tc attention: T=%d is not supported", T);
   const int Q = H * 64;
   TcOperand op, opv;
   int r = make_operand(&op, qkv_hi, qkv_lo, (uint64_t)B * T, (uint64_t)3 * Q, (uint64_t)3 * Q);
   if (r != MT3_OK) return r;
   r = make_operand(&opv, vt_hi, vt_lo, (uint64_t)B * H * 64, (uint64_t)T, (uint64_t)T, 64);
   if (r != MT3_OK) return r;
-  return launch_enc_attention_tc(op, opv, B, T, H, out_hi, out_lo, split3 != 0, 0, scratch);
+  return launch_attention_tc(op, 0, T, op, Q, T, opv, B, H, out_hi, out_lo, split3 != 0, false, false, nullptr, 0, 0, scratch);
 }
 
-KH_API long long kh_enc_attention_tc_scratch_floats(int B, int T, int H) { return (long long)enc_attention_tc_scratch_floats(B, T, H); }
-KH_API int kh_enc_attention_tc_supported(int T) { return enc_attention_tc_supported(T) ? 1 : 0; }
+KH_API long long kh_enc_attention_tc_scratch_floats(int B, int T, int H) { return (long long)attention_tc_scratch_floats(B, T, T, H, false); }
+KH_API int kh_enc_attention_tc_supported(int T) { return attention_tc_supported(T, T, false) ? 1 : 0; }
 
-// the exact-fp32 encoder attention
 KH_API int kh_enc_attention_fp32(const float* qkv, int B, int T, int H, float* out, float* out_lo) {
-  return launch_enc_attention(qkv, 3 * H * 64, T, H, B, out, out_lo, H * 64, 0);
+  const int Q = H * 64;
+  return launch_attention_fp32(qkv, 3 * Q, 0, qkv, 3 * Q, Q, 2 * Q, T, T, H, B, out, out_lo, Q, nullptr, 0, 0);
 }
 
 // The teacher-forced decoder's attention forms.  q [B*Tq, ldq] (head h at columns q_col0 + 64 h), k [B*Tk, ldk] (k_col0),
 // hi and lo; vt [B*H*64, Tk] (keys in vt_key_slot() order); out [B*Tq, H*64].  causal: Tq = Tk (a multiple of 128) and
-// key_valid [B, n_valid]; otherwise every key is visible.
+// key_valid [B, n_valid]; otherwise every key is visible.  P . V is split in TF32X3, as the pass runs it.
 KH_API int kh_attention_tc(const float* q_hi, const float* q_lo, int ldq, int q_col0, int Tq, const float* k_hi, const float* k_lo, int ldk,
                            int k_col0, int Tk, const float* vt_hi, const float* vt_lo, int B, int H, float* out_hi, float* out_lo, int split3,
                            int causal, const int* key_valid, int n_valid, float* scratch) {
@@ -114,8 +115,8 @@ KH_API int kh_attention_tc(const float* q_hi, const float* q_lo, int ldq, int q_
   if (r != MT3_OK) return r;
   r = make_operand(&ov, vt_hi, vt_lo, (uint64_t)B * H * 64, (uint64_t)Tk, (uint64_t)Tk, 64);
   if (r != MT3_OK) return r;
-  return launch_attention_tc(oq, q_col0, Tq, ok, k_col0, Tk, ov, B, H, out_hi, out_lo, split3 != 0, causal != 0, key_valid, n_valid, 0,
-                             scratch);
+  return launch_attention_tc(oq, q_col0, Tq, ok, k_col0, Tk, ov, B, H, out_hi, out_lo, split3 != 0, true, causal != 0, key_valid, n_valid,
+                             0, scratch);
 }
 KH_API long long kh_attention_tc_scratch_floats(int B, int Tq, int Tk, int H, int causal) {
   return (long long)attention_tc_scratch_floats(B, Tq, Tk, H, causal != 0);

@@ -35,7 +35,7 @@ EPI_STORE, EPI_RESIDUAL, EPI_ADD_PE, EPI_GATED_GELU = 0, 1, 2, 3
 # (2^-20 = 16 u)
 TOL_FP32 = 2.0 ** -17
 TOL_DEC = 2.0 ** -20
-# attention in fp32 (enc_attention_kernel, dec_attention_bulk_kernel): scores are 64-term dot products (tol_s), the
+# attention in fp32 (attention_fp32_kernel, dec_attention_bulk_kernel): scores are 64-term dot products (tol_s), the
 # weights carry expf's ulps and the row sum (tol_p)
 TOL_ENC_ATT_P, TOL_ENC_ATT_S = 2.0 ** -18, 2.0 ** -20
 TOL_DEC_ATT_P, TOL_DEC_ATT_S = 2.0 ** -20, 2.0 ** -22
@@ -438,7 +438,7 @@ def test_gemm_head_major_kv_store(kh, fmt, mode):
 
 
 # ------------------------------------------------------------------------------------------------
-# encoder attention: enc_attention_tc_kernel (+ combine) and the exact-fp32 enc_attention_kernel
+# encoder attention: attention_tc_kernel (+ combine) and the exact-fp32 attention_fp32_kernel in the encoder's form
 # ------------------------------------------------------------------------------------------------
 def _attn_inputs(rng, B, T, H, sharp):
     """qkv [B*T, 3*H*64] exactly as the QKV GEMM leaves it.  Diffuse: |S| ~ 1.  Sharp: S = r_i s_j along a shared
@@ -499,7 +499,7 @@ TOL_ATT_PV = {True: TOL_ATT_P, False: TOL_ATT_P}
     (512, 2, 2, True, True, True), (768, 2, 2, True, True, True), (1024, 2, 1, True, True, False), (1024, 1, 2, False, False, True),
     (256, 32, 6, False, True, True)])
 def test_enc_attention_tc(kh, T, B, H, sharp, split3, lo):
-    """enc_attention_tc_kernel: partial query tiles and masked keys (T = 8, 24, 72, 136, 200), one and two key chunks,
+    """attention_tc_kernel in the encoder's form: partial query tiles and masked keys (T = 8, 24, 72, 136, 200), one and two key chunks,
     the key-split form with KS = 2, 3, 4 (T = 512, 768, 1024) and its combine kernel, 2 .. 768 work items (below and far
     above the SM count: the persistent loop's barrier parity over many items per CTA), both precisions, out_lo null and
     not.  Measured worst err/bound: 3xTF32 0.21, TF32 0.18."""
@@ -510,7 +510,7 @@ def test_enc_attention_tc(kh, T, B, H, sharp, split3, lo):
 
 
 def enc_attention_tc_check(kh, qkv, B, T, H, split3, lo, name):
-    """enc_attention_tc_kernel on qkv [B*T, 3*H*64] against _attn_ref, per-element bars, NaN-poisoned outputs."""
+    """attention_tc_kernel (encoder form) on qkv [B*T, 3*H*64] against _attn_ref, per-element bars, NaN-poisoned outputs."""
     Q = H * 64
     vt = _vt_host(qkv, B, T, H)
     o_ref, cond_p, cond_s = _attn_ref(qkv, B, T, H)
@@ -538,7 +538,7 @@ def enc_attention_tc_check(kh, qkv, B, T, H, split3, lo, name):
 
 @pytest.mark.parametrize("T", [1, 37, 100, 300, 768])
 def test_enc_attention_fp32(kh, T):
-    """enc_attention_kernel (exact fp32; every T, the path of T % 8 != 0 and of T > 256 that is not a multiple of 256).
+    """attention_fp32_kernel in the encoder's form (exact fp32; every T, the path of T % 8 != 0 and of T > 256 that is not a multiple of 256).
     Measured worst err/bound: 0.22."""
     B, H = 2, 2
     rng = np.random.default_rng(T)
@@ -546,7 +546,7 @@ def test_enc_attention_fp32(kh, T):
 
 
 def enc_attention_fp32_check(kh, qkv, B, T, H, name):
-    """enc_attention_kernel on qkv [B*T, 3*H*64] (rows past B*T NaN), with and without out_lo, against _attn_ref."""
+    """attention_fp32_kernel (encoder form) on qkv [B*T, 3*H*64] (rows past B*T NaN), with and without out_lo, against _attn_ref."""
     Q = H * 64
     o_ref, cond_p, cond_s = _attn_ref(qkv, B, T, H)
     buf = _nan(B * T + 8, 3 * Q)                               # rows past B*T: NaN the kernel must not read
