@@ -181,6 +181,21 @@ enum {
 int mt3_generate(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                  int32_t* steps_run, void* stream);
 
+/* mt3_generate with the scores of T5X's predict_batch_with_aux: the same tokens, bit for bit, and
+ *   token_scores_out DEV f32 [B, max_decode_length] (may be NULL): the log-probability in float32,
+ *     logits[next] - logsumexp(logits row), of every emitted token, from the logits row that chose it.
+ *     Greedy: every token up to and including the first EOS; 0 for the PAD after it and beyond the steps run.
+ *     MT3_GEN_BEAM1: the returned hypothesis's -- its prefix, the EOS at position n - 1, 0 from n on (n = its
+ *     length); the live prefix when nothing finished.
+ *   scores_out DEV f32 [B] (may be NULL): greedy, the sum of the row's token scores in one fixed order;
+ *     MT3_GEN_BEAM1, T5X beam_search's score: log-probability / ((5 + n) / 6)^0.6 of the best finished
+ *     hypothesis, or the live log-probability when nothing finished.
+ * A logits row with a NaN gives a NaN token score, and the NaN carries into the sequence score.  With both
+ * outputs NULL this is mt3_generate; otherwise each step does one more reduction over its logits row (greedy)
+ * or a few more stores (beam1), in CUDA graphs of their own. */
+int mt3_generate_scored(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
+                        float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream);
+
 /* Transformer.decode(decode=False) / Transformer.__call__ (network.py:303-409 with decode=False, :196-262) and the token
  * scores of T5X's EncoderDecoderModel.score_batch (z_loss = 0): the teacher-forced decoder pass over all L positions at
  * once, from the caller's `encoded` DEV f32 [B, T, emb_dim] (the output of mt3_encode).

@@ -264,6 +264,33 @@ inline int launch_embed(const int* tok, const float* emb, int D, int vocab, cons
 }
 
 // ---------------------------------------------------------------------------------
+// logsumexp(x[0 .. V)) in a CTA of 256 threads, the one log-sum-exp of the greedy token scores and of the teacher-forced
+// token scores, so that one logits row gives the same bits in both: the row maximum (fmaxf, so NaN is skipped), then
+// sum expf(x - max) per thread in id order, a warp tree and the 8 warp sums in order.  A NaN in the row makes the sum, and
+// the result, NaN.  Every thread calls it (it synchronises the CTA) and every thread gets the result.  red: 8 shared floats.
+// ---------------------------------------------------------------------------------
+__device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, int V, float* red) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float mx = -INFINITY;
+  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
+  mx = warp_max(mx);
+  if (lane == 0) red[warp] = mx;
+  __syncthreads();
+  mx = red[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
+  __syncthreads();
+  float se = 0.f;
+  for (int c = tid; c < V; c += 256) se += expf(x[c] - mx);
+  se = warp_sum(se);
+  if (lane == 0) red[warp] = se;
+  __syncthreads();
+  float tot = 0.f;
+  for (int w = 0; w < 8; ++w) tot += red[w];
+  return mx + logf(tot);
+}
+
+// ---------------------------------------------------------------------------------
 // Greedy pick + loop bookkeeping (stands in for t5x's decode loop at num_decodes=1,
 // models.py:127): next = argmax(logits), like np/jnp.argmax: the first maximum wins, and
 // the first NaN wins over every number (tracked apart from the maximum, so the common
@@ -271,14 +298,16 @@ inline int launch_embed(const int* tok, const float* emb, int D, int vocab, cons
 // (id 1, vocabularies.py:157-159) marks finished.
 // The last CTA to arrive advances the shared position and publishes all_finished.
 // state: [0] pos, [1] arrival counter, [2] all_finished
+// token_scores (optional, row stride out_ld): [b, pos] = logits[next] - logsumexp(logits row) (block_logsumexp), 0 for a
+// sequence that had finished before this step (it emits PAD); NaN when the row holds a NaN.
 // y_next (optional) = E[next] + PE[pos + 1], skipped at the last step, where pos + 1 = pe_rows has no PE row.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
-                   int* __restrict__ finished, int* __restrict__ tokens_out, int out_ld, int* __restrict__ tok_out_user,
-                   int* __restrict__ state, int advance, int b0, const float* __restrict__ emb, const float* __restrict__ pe,
-                   int pe_rows, int D, float* __restrict__ y_next) {
-  __shared__ float sv[8];
+                   int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
+                   int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0, const float* __restrict__ emb,
+                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+  __shared__ float sv[8], slse[8];
   __shared__ int si[8], snan[8];
   __shared__ int s_next[2];
   pdl_wait();
@@ -304,6 +333,7 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
   nan_i = __reduce_min_sync(0xffffffffu, nan_i);
   if (lane == 0) { sv[warp] = best; si[warp] = bi; snan[warp] = nan_i; }
   __syncthreads();
+  const float lse = token_scores ? block_logsumexp(l, V, slse) : 0.f;
   if (tid == 0) {
     for (int w = 1; w < 8; ++w) {
       if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
@@ -312,14 +342,16 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
     if (nan_i != 0x7fffffff) bi = nan_i;
     const int pos = state[0];
     int nxt = bi;
+    float lp = token_scores ? l[bi] - lse : 0.f;
     if (finished) {
-      if (finished[b]) nxt = 0;
+      if (finished[b]) { nxt = 0; lp = 0.f; }
       if (nxt == 1) finished[b] = 1;
     }
     s_next[0] = nxt;
     s_next[1] = pos + 1;
     if (tok_cur) tok_cur[b] = nxt;
     if (tokens_out) tokens_out[(long long)b * out_ld + pos] = nxt;
+    if (token_scores) token_scores[(long long)b * out_ld + pos] = lp;
     if (tok_out_user) tok_out_user[b] = nxt;
     if (advance) {
       __threadfence();
@@ -356,11 +388,11 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
 }
 
 // sequences b0 .. b0 + n_cta - 1 of a batch of B
-inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld,
-                              int* tok_out_user, int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows,
-                              int D, float* y_next, int n_cta, cudaStream_t s) {
+inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                              int out_ld, int* tok_out_user, int* state, int advance, int b0, const float* emb, const float* pe,
+                              int pe_rows, int D, float* y_next, int n_cta, cudaStream_t s) {
   MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
-                               out_ld, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
+                               token_scores, out_ld, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -380,6 +412,8 @@ inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, i
 // score is NaN).  A row that is only partly NaN makes the log-sum-exp NaN; what T5X does then depends on its NaN
 // ordering, which is not pinned here, so such rows carry no parity claim.
 // beam_f [B][2] = {live_lp, finished score}, beam_i [B] = length of the best finished hypothesis (0 = none yet).
+// token_scores (optional, row stride out_ld): [b, pos] = the live token's log-probability v1 - lse; with it, fin_lp_eos [B]
+// keeps the EOS log-probability of the best finished hypothesis, which beam1_finalize_kernel puts at its last position.
 // y_next as in argmax_step_kernel.
 // ---------------------------------------------------------------------------------
 // Candidate order: larger value first, NaN above every number, lower id first among equals (and among NaNs).  The
@@ -391,9 +425,9 @@ __device__ __forceinline__ bool cand_better(float v, int i, float ov, int oi) {
 
 __global__ void __launch_bounds__(256)
 beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
-                  int* __restrict__ tokens_out, int out_ld, int* __restrict__ state, float* __restrict__ beam_f,
-                  int* __restrict__ beam_i, float alpha, int max_len, const float* __restrict__ emb, const float* __restrict__ pe,
-                  int pe_rows, int D, float* __restrict__ y_next) {
+                  int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, int* __restrict__ state,
+                  float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
+                  const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
   __shared__ float s1v[8], s2v[8], smx[8], ssum[8];
   __shared__ int s1i[8], s2i[8];
   __shared__ int s_next[2];
@@ -454,12 +488,14 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
         fin_score = cand;
         beam_f[2 * b + 1] = cand;
         beam_i[b] = pos + 1;
+        if (token_scores) fin_lp_eos[b] = veos - lse;
       }
     }
     const float live = live_prev + (v1 - lse);
     beam_f[2 * b] = live;
     tok_cur[b] = i1;
     tokens_out[(long long)b * out_ld + pos] = i1;
+    if (token_scores) token_scores[(long long)b * out_ld + pos] = v1 - lse;
     finished[b] = (beam_i[b] > 0 && fin_score > live / powf((5.0f + (float)max_len) / 6.0f, alpha)) ? 1 : 0;
     s_next[0] = i1;
     s_next[1] = pos + 1;
@@ -488,30 +524,59 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
   }
 }
 
-inline int launch_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
-                             float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
-                             float* y_next, cudaStream_t s) {
-  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out, out_ld,
-                               state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
+inline int launch_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                             int out_ld, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha, int max_len,
+                             const float* emb, const float* pe, int pe_rows, int D, float* y_next, cudaStream_t s) {
+  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
+                               token_scores, out_ld, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
 
 // the best finished hypothesis = the live prefix up to its finish + EOS, zeros after; a sequence that never finished keeps
-// its live tokens (the reference returns the live beam when nothing finished)
-__global__ void beam1_finalize_kernel(int* __restrict__ tokens, int B, int L, int steps, const int* __restrict__ beam_i) {
+// its live tokens (the reference returns the live beam when nothing finished).
+// token_scores (optional, [B, L], as beam1_step_kernel wrote them) get the same cut: fin_lp_eos[b] at n - 1, zeros after.
+// scores (optional, [B]) = T5X beam_search's score: the best finished score of beam_f, or the live log-probability when
+// nothing finished.
+__global__ void beam1_finalize_kernel(int* __restrict__ tokens, int B, int L, int steps, const int* __restrict__ beam_i,
+                                      float* __restrict__ token_scores, const float* __restrict__ beam_f,
+                                      const float* __restrict__ fin_lp_eos, float* __restrict__ scores) {
   const int b = blockIdx.x;
   const int n = beam_i[b];
-  if (n <= 0) {
-    for (int i = steps + threadIdx.x; i < L; i += blockDim.x) tokens[(long long)b * L + i] = 0;
-    return;
+  if (scores && threadIdx.x == 0) scores[b] = n > 0 ? beam_f[2 * b + 1] : beam_f[2 * b];
+  const int from = n > 0 ? n : steps;
+  if (n > 0 && threadIdx.x == 0) {
+    tokens[(long long)b * L + n - 1] = 1;
+    if (token_scores) token_scores[(long long)b * L + n - 1] = fin_lp_eos[b];
   }
-  if (threadIdx.x == 0) tokens[(long long)b * L + n - 1] = 1;
-  for (int i = n + threadIdx.x; i < L; i += blockDim.x) tokens[(long long)b * L + i] = 0;
+  for (int i = from + threadIdx.x; i < L; i += blockDim.x) {
+    tokens[(long long)b * L + i] = 0;
+    if (token_scores) token_scores[(long long)b * L + i] = 0.f;
+  }
 }
 
-inline int launch_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i, cudaStream_t s) {
-  beam1_finalize_kernel<<<B, 128, 0, s>>>(tokens, B, L, steps, beam_i);
+inline int launch_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i, float* token_scores, const float* beam_f,
+                                 const float* fin_lp_eos, float* scores, cudaStream_t s) {
+  beam1_finalize_kernel<<<B, 128, 0, s>>>(tokens, B, L, steps, beam_i, token_scores, beam_f, fin_lp_eos, scores);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// scores[b] = the sum of token_scores[b, 0 .. L) (greedy sequence score), in one fixed order whatever the steps ran: each
+// of 128 threads sums ids tid, tid + 128, ... in order, then a warp tree and the 4 warp sums in order.
+__global__ void __launch_bounds__(128) seq_score_kernel(const float* __restrict__ token_scores, int L, float* __restrict__ scores) {
+  __shared__ float red[4];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  float s = 0.f;
+  for (int i = tid; i < L; i += 128) s += token_scores[(long long)b * L + i];
+  s = warp_sum(s);
+  if ((tid & 31) == 0) red[tid >> 5] = s;
+  __syncthreads();
+  if (tid == 0) scores[b] = ((red[0] + red[1]) + red[2]) + red[3];
+}
+
+inline int launch_seq_score(const float* token_scores, int B, int L, float* scores, cudaStream_t s) {
+  seq_score_kernel<<<B, 128, 0, s>>>(token_scores, L, scores);
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -681,7 +746,7 @@ token_score_kernel(const float* __restrict__ logits, int V, int row0, int Lp, in
   const int g = row0 + blockIdx.x;
   const int b = g / Lp, i = g % Lp;
   if (i >= L) return;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const float* x = logits + (long long)blockIdx.x * V;
   const long long pos = (long long)b * L + i;
   if (logits_out) {
@@ -690,27 +755,12 @@ token_score_kernel(const float* __restrict__ logits, int V, int row0, int Lp, in
     for (int c = tid; c < V / 4; c += 256) dst[c] = src[c];
   }
   if (!scores) return;
-  float mx = -INFINITY;
-  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
-  mx = warp_max(mx);
-  if (lane == 0) red[warp] = mx;
-  __syncthreads();
-  mx = red[0];
-#pragma unroll
-  for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
-  __syncthreads();
-  float se = 0.f;
-  for (int c = tid; c < V; c += 256) se += expf(x[c] - mx);
-  se = warp_sum(se);
-  if (lane == 0) red[warp] = se;
-  __syncthreads();
+  const float lse = block_logsumexp(x, V, red);
   if (tid == 0) {
-    float tot = 0.f;
-    for (int w = 0; w < 8; ++w) tot += red[w];
     const int tg = target[pos];
     const float wt = weight ? (float)weight[pos] : (tg > 0 ? 1.f : 0.f);
     const int t = min(max(tg, 0), V - 1);
-    scores[pos] = wt != 0.f ? (x[t] - (mx + logf(tot))) * wt : 0.f;
+    scores[pos] = wt != 0.f ? (x[t] - lse) * wt : 0.f;
   }
 }
 

@@ -130,6 +130,8 @@ struct Model {
   int *tok_cur = nullptr, *finished = nullptr, *tokens = nullptr, *state = nullptr;
   float* att_scratch = nullptr;   // key-split encoder attention (T > 256): unnormalised O parts + (max, sum) pairs
   float* beam_f = nullptr; int* beam_i = nullptr;   // beam-size-1 search state (MT3_GEN_BEAM1)
+  float* fin_lp_eos = nullptr;    // [B] EOS log-probability of each best finished hypothesis (beam_f's third float per sequence)
+  float *tok_scores = nullptr, *seq_scores = nullptr;   // [B, L] and [B] of mt3_generate_scored
   float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
   int dcounters_n = 0;
   int* dcounters = nullptr;
@@ -495,8 +497,9 @@ static int dec_layer_mlp(Model* m, const DecBranch& b, int l, cudaStream_t s) {
 // [norm+gated-GELU MLP in] [MLP out+residual].
 // loop_step: a step of mt3_generate's loop -- the decoder input m->dy was already written (by dec_embed before the first
 // step, by the previous step's argmax kernel afterwards), and this step's argmax kernel writes the next one.
+// scored: the token picker also writes each emitted token's log-probability to m->tok_scores (mt3_generate_scored).
 static int decode_step_impl(Model* m, const int* tok_in, float* logits, int greedy, int* tok_user, int use_finished,
-                            int* tokens_ws, cudaStream_t s, bool loop_step = false) {
+                            int* tokens_ws, cudaStream_t s, bool loop_step = false, bool scored = false) {
   if (!loop_step) MT3_TRY(dec_embed(m, tok_in, s));
   DecBranch b{m->dy, false};
   for (int l = 0; l < m->Ld; ++l) {
@@ -509,12 +512,13 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
   MT3_TRY(dec_gemm(m, "gemm_logits", b.y, m->D, m->w_logits, m->V, m->D, 1, EPI_STORE, logits, m->V, m->V, nullptr, nullptr, s,
                    kv_stage_for(m, 0, 1), dec_chain(m, true, false)));
   float* y_next = loop_step ? m->dy : nullptr;
+  float* tok_scores = scored ? m->tok_scores : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
-    MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, m->L, m->state, m->beam_f, m->beam_i, 0.6f, m->L,
-                              m->emb, m->pe, m->pe_rows, m->D, y_next, s));
+    MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->state, m->beam_f, m->fin_lp_eos,
+                              m->beam_i, 0.6f, m->L, m->emb, m->pe, m->pe_rows, m->D, y_next, s));
   } else if (greedy) {
     MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
-                               m->L, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D, y_next, m->B, s));
+                               tok_scores, m->L, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D, y_next, m->B, s));
   } else {
     MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
     MT3_LAUNCH_CHECK();
@@ -544,9 +548,10 @@ static void select_graph(Model* m, int mode = 1) {
 }
 
 // mode: 1 greedy, 2 beam-size-1 search; nsteps consecutive decode steps per graph (the position lives on the device, so a
-// graph of 16 steps is the single-step graph 16 times over: one graph launch and its ~3 us of inter-launch latency per 16 steps)
-static int ensure_graph(Model* m, int mode, int nsteps = 1) {
-  const int key = mode | (nsteps << 8);
+// graph of 16 steps is the single-step graph 16 times over: one graph launch and its ~3 us of inter-launch latency per 16 steps);
+// scored: the token pickers write token scores (a graph of its own, so that the unscored graphs do no extra work)
+static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
+  const int key = mode | (scored ? 4 : 0) | (nsteps << 8);
   if (m->graph_mode != key) select_graph(m, key);
   if (m->graph_exec) return MT3_OK;
   if (!m->cap_stream) MT3_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
@@ -554,7 +559,7 @@ static int ensure_graph(Model* m, int mode, int nsteps = 1) {
   MT3_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
   int r = MT3_OK;
   for (int i = 0; i < nsteps && r == MT3_OK; ++i)
-    r = decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, m->cap_stream, true);
+    r = decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, m->cap_stream, true, scored);
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaStreamEndCapture(m->cap_stream, &g);
   if (r != MT3_OK) {
@@ -566,11 +571,19 @@ static int ensure_graph(Model* m, int mode, int nsteps = 1) {
   m->graph_kernels = g_launch_count.load() - before;
   g_launch_count.fetch_sub(m->graph_kernels);   // capture does not execute
   MT3_CUDA_CHECK(cudaGraphInstantiate(&m->graph_exec, m->graph, 0));
-  if (m->graphs.size() >= 12) {                 // bound the cache: forget everything but the new graph
-    const Model::StepGraph keep{m->graph, m->graph_exec, m->graph_kernels};
-    m->graph = nullptr; m->graph_exec = nullptr;
-    drop_graphs(m);
-    m->graph = keep.g; m->graph_exec = keep.e; m->graph_kernels = keep.kernels;
+  // bound the cache: forget the graphs of other (workspace, B, T) bindings.  The current binding's stay: it has at most 8
+  // (2 modes x scored or not x 1 or 16 steps), and a caller may still hold one of them (mt3_generate_scored keeps the
+  // 16-step graph while it makes sure of the single-step one).
+  if (m->graphs.size() >= 12) {
+    for (auto it = m->graphs.begin(); it != m->graphs.end();) {
+      if (std::get<0>(it->first) != (const void*)m->ws || std::get<1>(it->first) != m->B || std::get<2>(it->first) != m->T) {
+        cudaGraphExecDestroy(it->second.e);
+        cudaGraphDestroy(it->second.g);
+        it = m->graphs.erase(it);
+      } else {
+        ++it;
+      }
+    }
   }
   m->graphs[std::make_tuple((const void*)m->ws, m->B, m->T, key)] = Model::StepGraph{m->graph, m->graph_exec, m->graph_kernels};
   return MT3_OK;
@@ -923,7 +936,8 @@ namespace {
 struct WsLayout {
   int64_t x_hi, x_lo, h_lo, ao_lo, g_lo, enc_hi, enc_lo, qkv_lo, vt_hi, vt_lo;
   int64_t dy2, dssq;
-  int64_t h, rstd, qkv, ao, g, encoded, ckv, skv, dy, drstd, dq, dao, dg, dlogits, tok_cur, finished, tokens, state, dpartial, dcounters, beam_f, beam_i, att_scratch, total;
+  int64_t h, rstd, qkv, ao, g, encoded, ckv, skv, dy, drstd, dq, dao, dg, dlogits, tok_cur, finished, tokens, state, dpartial, dcounters, beam_f, beam_i, att_scratch;
+  int64_t tok_scores, seq_scores, total;
 };
 WsLayout ws_layout(const Model* m, int B, int T) {
   WsLayout w;
@@ -964,8 +978,10 @@ WsLayout ws_layout(const Model* m, int B, int T) {
   w.dpartial = take((int64_t)16 * cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * kDecTileFloats * 4);   // up to 16 K chunks
   w.dcounters = take((int64_t)cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * 4);
   w.att_scratch = take(m->tc ? attention_tc_scratch_floats(B, T, T, m->H, false) * 4 : 0);
-  w.beam_f = take((int64_t)B * 2 * 4);
+  w.beam_f = take((int64_t)B * 3 * 4);      // {live_lp, finished score} per sequence, then fin_lp_eos [B]
   w.beam_i = take((int64_t)B * 4);
+  w.tok_scores = take((int64_t)B * L * 4);
+  w.seq_scores = take((int64_t)B * 4);
   w.total = off;
   return w;
 }
@@ -995,7 +1011,8 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
   m->dg = (float*)(b + w.dg); m->dlogits = (float*)(b + w.dlogits); m->tok_cur = (int*)(b + w.tok_cur);
   m->finished = (int*)(b + w.finished); m->tokens = (int*)(b + w.tokens); m->state = (int*)(b + w.state);
   m->dpartial = (float*)(b + w.dpartial); m->dcounters = (int*)(b + w.dcounters);
-  m->beam_f = (float*)(b + w.beam_f); m->beam_i = (int*)(b + w.beam_i);
+  m->beam_f = (float*)(b + w.beam_f); m->beam_i = (int*)(b + w.beam_i); m->fin_lp_eos = m->beam_f + 2 * batch;
+  m->tok_scores = (float*)(b + w.tok_scores); m->seq_scores = (float*)(b + w.seq_scores);
   const bool key_split = m->tc && attention_tc_scratch_floats(batch, input_length, input_length, m->H, false) > 0;
   m->att_scratch = key_split ? (float*)(b + w.att_scratch) : nullptr;
   m->dcounters_n = cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN);
@@ -1042,17 +1059,22 @@ extern "C" int mt3_decode_step(mt3_model* h, const int32_t* tok_in, float* logit
                           (cudaStream_t)stream);
 }
 
-extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
-                            int32_t* steps_run, void* stream) {
-  MT3_REQUIRE(h && x && tokens_out, MT3_ERR_BAD_ARG, "mt3_generate: null argument");
+// mt3_generate and mt3_generate_scored; `name` is the entry point the caller used, for its error messages
+static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
+                         float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream) {
+  MT3_REQUIRE(h && x && tokens_out, MT3_ERR_BAD_ARG, "%s: null argument", name);
   Model* m = reinterpret_cast<Model*>(h);
   MT3_NEED_WS(m);
-  MT3_REQUIRE(num_steps >= 0 && num_steps <= m->L, MT3_ERR_SHAPE, "num_steps %d outside [0, max_decode_length=%d]", num_steps, m->L);
-  MT3_REQUIRE((flags & ~(MT3_GEN_STOP_AT_EOS | MT3_GEN_USE_GRAPH | MT3_GEN_BEAM1)) == 0, MT3_ERR_BAD_ARG, "mt3_generate: unknown flag bits 0x%x", flags);
+  MT3_REQUIRE(num_steps >= 0 && num_steps <= m->L, MT3_ERR_SHAPE, "%s: num_steps %d outside [0, max_decode_length=%d]", name, num_steps,
+              m->L);
+  MT3_REQUIRE((flags & ~(MT3_GEN_STOP_AT_EOS | MT3_GEN_USE_GRAPH | MT3_GEN_BEAM1)) == 0, MT3_ERR_BAD_ARG, "%s: unknown flag bits 0x%x", name,
+              flags);
   cudaStream_t s = (cudaStream_t)stream;
   MT3_TRY(encode_impl(m, x, m->encoded, s));
   MT3_TRY(cross_kv_impl(m, m->encoded, s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
+  const bool scored = token_scores_out || scores_out;
+  if (scored) MT3_CUDA_CHECK(cudaMemsetAsync(m->tok_scores, 0, (size_t)m->B * m->L * sizeof(float), s));
   const bool use_graph = (flags & MT3_GEN_USE_GRAPH) != 0;
   const bool stop = (flags & MT3_GEN_STOP_AT_EOS) != 0;
   const int mode = (flags & MT3_GEN_BEAM1) ? 2 : 1;
@@ -1068,11 +1090,11 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
   uint64_t k1 = 0, kN = 0;
   if (use_graph) {
     if (num_steps >= kBlock) {
-      MT3_TRY(ensure_graph(m, mode, kBlock));
+      MT3_TRY(ensure_graph(m, mode, kBlock, scored));
       gN = m->graph_exec; kN = m->graph_kernels;
     }
     if (num_steps % kBlock != 0) {
-      MT3_TRY(ensure_graph(m, mode, 1));
+      MT3_TRY(ensure_graph(m, mode, 1, scored));
       g1 = m->graph_exec; k1 = m->graph_kernels;
     }
   }
@@ -1089,7 +1111,7 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
       MT3_CUDA_CHECK(cudaGraphLaunch(g1, s));
       count_launch(k1);
     } else {
-      MT3_TRY(decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, s, true));
+      MT3_TRY(decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, s, true, scored));
     }
     step += n;
     ran += n;
@@ -1101,11 +1123,27 @@ extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int
     }
   }
   if (mode == 2) {
-    MT3_TRY(launch_beam1_finalize(m->tokens, m->B, m->L, ran, m->beam_i, s));
+    MT3_TRY(launch_beam1_finalize(m->tokens, m->B, m->L, ran, m->beam_i, scored ? m->tok_scores : nullptr, m->beam_f, m->fin_lp_eos,
+                                  scored ? m->seq_scores : nullptr, s));
+  } else if (scored) {
+    MT3_TRY(launch_seq_score(m->tok_scores, m->B, m->L, m->seq_scores, s));
   }
   MT3_CUDA_CHECK(cudaMemcpyAsync(tokens_out, m->tokens, (size_t)m->B * m->L * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  if (token_scores_out)
+    MT3_CUDA_CHECK(cudaMemcpyAsync(token_scores_out, m->tok_scores, (size_t)m->B * m->L * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (scores_out) MT3_CUDA_CHECK(cudaMemcpyAsync(scores_out, m->seq_scores, (size_t)m->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
   if (steps_run) *steps_run = ran;
   return MT3_OK;
+}
+
+extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
+                            int32_t* steps_run, void* stream) {
+  return generate_impl("mt3_generate", h, x, num_steps, flags, tokens_out, nullptr, nullptr, steps_run, stream);
+}
+
+extern "C" int mt3_generate_scored(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
+                                   float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream) {
+  return generate_impl("mt3_generate_scored", h, x, num_steps, flags, tokens_out, token_scores_out, scores_out, steps_run, stream);
 }
 
 extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length, int32_t target_length) {

@@ -165,19 +165,44 @@ KH_API int kh_p24_roundtrip(const float* x, float* y, uint32_t* code, long long 
 KH_API int kh_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* tok_user,
                           int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows, int D, float* y_next,
                           int n_cta) {
-  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows, D, y_next,
-                            n_cta, 0);
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows,
+                            D, y_next, n_cta, 0);
 }
 
 KH_API int kh_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
                          float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
                          float* y_next) {
-  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, out_ld, state, beam_f, beam_i, alpha, max_len, emb, pe, pe_rows, D,
-                           y_next, 0);
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, state, beam_f, nullptr, beam_i, alpha, max_len,
+                           emb, pe, pe_rows, D, y_next, 0);
 }
 
 KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i) {
-  return launch_beam1_finalize(tokens, B, L, steps, beam_i, 0);
+  return launch_beam1_finalize(tokens, B, L, steps, beam_i, nullptr, nullptr, nullptr, nullptr, 0);
+}
+
+// The same kernels with token scores (mt3_generate_scored): token_scores [B, out_ld] (row stride out_ld, like tokens_out),
+// fin_lp_eos [B], scores [B]; beam_f [B][2] as above.
+KH_API int kh_argmax_step_scored(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                 int out_ld, int* tok_user, int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows,
+                                 int D, float* y_next, int n_cta) {
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, tok_user, state, advance, b0, emb, pe,
+                            pe_rows, D, y_next, n_cta, 0);
+}
+
+KH_API int kh_beam1_step_scored(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                int out_ld, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha, int max_len,
+                                const float* emb, const float* pe, int pe_rows, int D, float* y_next) {
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, state, beam_f, fin_lp_eos, beam_i, alpha,
+                           max_len, emb, pe, pe_rows, D, y_next, 0);
+}
+
+KH_API int kh_beam1_finalize_scored(int* tokens, int B, int L, int steps, const int* beam_i, float* token_scores, const float* beam_f,
+                                    const float* fin_lp_eos, float* scores) {
+  return launch_beam1_finalize(tokens, B, L, steps, beam_i, token_scores, beam_f, fin_lp_eos, scores, 0);
+}
+
+KH_API int kh_seq_score(const float* token_scores, int B, int L, float* scores) {
+  return launch_seq_score(token_scores, B, L, scores, 0);
 }
 
 // y [b0 + n, D] rows b0 .. b0 + n - 1

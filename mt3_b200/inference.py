@@ -167,10 +167,12 @@ class InferenceModel(object):
         return self.vocabulary.decode_tf(prediction).cpu().numpy()
 
     def transcribe_segments(self, audio_segments, n_valid_frames=None, num_steps: Optional[int] = None,
-                            stop_at_eos: bool = True, decoded: bool = True) -> np.ndarray:
+                            stop_at_eos: bool = True, decoded: bool = True, return_scores: bool = False):
         """Hot path end to end for already-cut segments: host float32 [S, inputs_length*hop] ->
         host int32 [S, 1024].  H2D copy, log-mel kernel, encoder, greedy decoder, (vocab decode),
-        D2H copy; batches of `batch_size`.  This is the call bench.py's `e2e` times."""
+        D2H copy; batches of `batch_size`.  This is the call bench.py's `e2e` times.
+        return_scores=True returns (tokens, token_scores float32 [S, 1024], scores float32 [S]) with the same tokens: how sure
+        the model was of each emitted token (its log-probability; 0 after EOS) and of each segment (Transformer.generate)."""
         a = audio_segments
         if isinstance(a, np.ndarray):
             a = torch.from_numpy(a)
@@ -179,6 +181,9 @@ class InferenceModel(object):
             a = a.pin_memory()              # so that the per-batch H2D copies below are truly asynchronous
         S = a.shape[0]
         out = torch.empty((S, self.outputs_length), dtype=torch.int32, pin_memory=True)
+        if return_scores:
+            out_ts = torch.empty((S, self.outputs_length), dtype=torch.float32, pin_memory=True)
+            out_sc = torch.empty((S,), dtype=torch.float32, pin_memory=True)
         nv = None
         if n_valid_frames is not None:
             nv = torch.as_tensor(n_valid_frames, dtype=torch.int32).to(self.device)
@@ -189,17 +194,24 @@ class InferenceModel(object):
                                                     n_valid_frames=None if nv is None else nv[s0:s1])
             spec = self._pad_inputs(spec)
             toks = self.model.generate(spec, num_steps=num_steps, stop_at_eos=stop_at_eos, use_graph=self.use_graph,
-                                       decode=self.decode)
+                                       decode=self.decode, return_scores=return_scores)
+            if return_scores:
+                toks, ts, sc = toks
+                out_ts[s0:s1].copy_(ts, non_blocking=True)
+                out_sc[s0:s1].copy_(sc, non_blocking=True)
             if decoded:
                 toks = self.vocabulary.decode_tf(toks)
             out[s0:s1].copy_(toks, non_blocking=True)
         torch.cuda.synchronize(self.device)
+        if return_scores:
+            return out.numpy(), out_ts.numpy(), out_sc.numpy()
         return out.numpy()
 
-    def transcribe_segments_sharded(self, audio_segments, **kwargs) -> np.ndarray:
+    def transcribe_segments_sharded(self, audio_segments, **kwargs):
         """Data-parallel transcribe_segments (SURVEY 8e): every rank passes the SAME global segment
         list, transcribes its contiguous shard on its own GPU and receives all token streams
-        int32 [S, 1024] in segment order after ONE all-gather.  Identity with a single process."""
+        int32 [S, 1024] in segment order after ONE all-gather (three with return_scores=True: tokens, token scores
+        and scores, as transcribe_segments returns them).  Identity with a single process."""
         from . import distributed as mt3_dist
         rank, world_size = mt3_dist.world()
         a = audio_segments
@@ -212,12 +224,18 @@ class InferenceModel(object):
         nv = kwargs.pop('n_valid_frames', None)
         if nv is not None:
             nv = np.asarray(nv)[lo:hi]
+        scored = kwargs.get('return_scores', False)
         if hi > lo:
-            local = torch.from_numpy(self.transcribe_segments(a[lo:hi], n_valid_frames=nv, **kwargs))
+            local = self.transcribe_segments(a[lo:hi], n_valid_frames=nv, **kwargs)
         else:
-            local = torch.empty((0, self.outputs_length), dtype=torch.int32)
-        gathered = mt3_dist.gather_tokens(local.to(self.device), S)
-        return gathered.cpu().numpy()
+            empty = np.zeros((0, self.outputs_length), np.int32)
+            local = (empty, empty.astype(np.float32), np.zeros((0,), np.float32)) if scored else empty
+        if not scored:
+            return mt3_dist.gather_tokens(torch.from_numpy(local).to(self.device), S).cpu().numpy()
+        toks, ts, sc = local
+        toks, ts, sc = (mt3_dist.gather_tokens(t.to(self.device), S).cpu().numpy()
+                        for t in (torch.from_numpy(toks), torch.from_numpy(ts), torch.from_numpy(sc)[:, None]))
+        return toks, ts, sc[:, 0]
 
     def _pad_inputs(self, spec: torch.Tensor) -> torch.Tensor:
         """Feature converter (models.py:96): trim/pad the frame axis to inputs_length with 0.0."""

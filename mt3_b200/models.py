@@ -14,6 +14,7 @@ the reference's model inherits): the log-likelihood of given targets, from the t
 """
 from __future__ import annotations
 
+import inspect
 from typing import Any, Dict, List, Mapping, Sequence
 
 import numpy as np
@@ -93,11 +94,7 @@ class ContinuousInputsEncoderDecoderModel:
             assert enc[-1] == self._input_depth
         return {**dict(input_shapes), 'encoder_input_tokens': enc}
 
-    def predict_batch_with_aux(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None, num_decodes: int = 1,
-                               return_all_decodes: bool = False):
-        """tokens int32 [B, max_decode_length] (0 after EOS) and an empty aux dict.  `params` is accepted for signature
-        fidelity: the weights live in the module."""
-        del params, rng, return_all_decodes
+    def _inputs(self, batch: Mapping[str, Any], decoder_params, num_decodes: int):
         if num_decodes != 1:
             raise ValueError('only num_decodes=1 is built (the notebook and infer.gin use the default)')
         if decoder_params and decoder_params.get('decode_rng') is not None:
@@ -105,10 +102,29 @@ class ContinuousInputsEncoderDecoderModel:
         x = batch['encoder_input_tokens']
         if x.shape[-1] != self._input_depth:
             raise ValueError('encoder_input_tokens depth %d != input_depth %d' % (x.shape[-1], self._input_depth))
-        return self.module.generate(x, stop_at_eos=True, decode=self._decode), {}
+        return x
+
+    def predict_batch_with_aux(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None, num_decodes: int = 1,
+                               return_all_decodes: bool = False):
+        """tokens int32 [B, max_decode_length] (0 after EOS) and T5X's aux dict {'scores': float32 [B]}: the greedy sequence's
+        summed token log-probabilities, or beam_search's length-normalised score.  A module whose `generate` cannot return
+        scores (no `return_scores` argument) gives an empty aux dict.  return_all_decodes=True adds T5X's decodes axis:
+        tokens [B, 1, max_decode_length], scores [B, 1].  `params` is accepted for signature fidelity: the weights live in
+        the module."""
+        del params, rng
+        x = self._inputs(batch, decoder_params, num_decodes)
+        aux = {}
+        if 'return_scores' in inspect.signature(self.module.generate).parameters:
+            tokens, _, scores = self.module.generate(x, stop_at_eos=True, decode=self._decode, return_scores=True)
+            aux['scores'] = scores[:, None] if return_all_decodes else scores
+        else:
+            tokens = self.module.generate(x, stop_at_eos=True, decode=self._decode)
+        return (tokens[:, None] if return_all_decodes else tokens), aux
 
     def predict_batch(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None):
-        return self.predict_batch_with_aux(params, batch, rng=rng, decoder_params=decoder_params)[0]
+        """The tokens of predict_batch_with_aux, without computing scores."""
+        del params, rng
+        return self.module.generate(self._inputs(batch, decoder_params, 1), stop_at_eos=True, decode=self._decode)
 
     def score_batch(self, params, batch: Mapping[str, Any], return_intermediates: bool = False):
         """T5X EncoderDecoderModel.score_batch with z_loss = 0: float32 [B], the sum over positions of

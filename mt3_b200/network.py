@@ -242,11 +242,14 @@ class Transformer:
         return torch.cat(outs, dim=1)
 
     def generate(self, encoder_input_tokens: torch.Tensor, num_steps: Optional[int] = None, stop_at_eos: bool = True,
-                 use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy') -> torch.Tensor:
+                 use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy', return_scores: bool = False):
         """encode + decode from BOS=0 (models.py:121-138).  decode='greedy': argmax until EOS; decode='beam1': T5X's
         decoding.beam_search at num_decodes=1, the reference's decode_fn (models.py:127) -- they differ when EOS is one of the
         two best tokens without being decisive (tests/test_beam1.py).  Returns raw model ids int32 [B, max_decode_length],
-        0 after EOS."""
+        0 after EOS.
+        return_scores=True returns (tokens, token_scores float32 [B, max_decode_length], scores float32 [B]) with the same
+        tokens: each emitted token's log-probability (0 after EOS and beyond the steps run) and the sequence score -- greedy,
+        the sum of the token scores; beam1, T5X beam_search's length-normalised score (mt3_generate_scored)."""
         if decode not in ('greedy', 'beam1'):
             raise ValueError("decode must be 'greedy' or 'beam1'")
         x = self._check_inputs(encoder_input_tokens)
@@ -258,7 +261,15 @@ class Transformer:
         flags = (_lib.GEN_STOP_AT_EOS if stop_at_eos else 0) | (_lib.GEN_USE_GRAPH if use_graph else 0) | \
                 (_lib.GEN_BEAM1 if decode == 'beam1' else 0)
         ran = C.c_int32(0)
+        if not return_scores:
+            with torch.cuda.device(self.device):
+                _lib.check(self._lib.mt3_generate(self._h, x.data_ptr(), steps, flags, out.data_ptr(), C.byref(ran), self._stream()))
+            self.last_steps_run = int(ran.value)
+            return out
+        token_scores = torch.empty((b, self.max_decode_length), dtype=torch.float32, device=self.device)
+        scores = torch.empty((b,), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self._lib.mt3_generate(self._h, x.data_ptr(), steps, flags, out.data_ptr(), C.byref(ran), self._stream()))
+            _lib.check(self._lib.mt3_generate_scored(self._h, x.data_ptr(), steps, flags, out.data_ptr(), token_scores.data_ptr(),
+                                                     scores.data_ptr(), C.byref(ran), self._stream()))
         self.last_steps_run = int(ran.value)
-        return out
+        return out, token_scores, scores
