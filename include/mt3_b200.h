@@ -219,6 +219,28 @@ int mt3_decode_teacher_forced(mt3_model* m, const float* encoded, int32_t batch,
                               const int32_t* loss_weights, int32_t target_length, float* logits, float* token_scores,
                               void* workspace, int64_t workspace_bytes, void* stream);
 
+/* mt3_generate_scored with a forced decoder prefix per sequence: T5X predict_batch_with_aux(prompt_with_targets=True).
+ *   prompt DEV i32 [B, prompt_len], 0 <= prompt_len <= num_steps: row b's prompt is its non-zero prefix, of length p_b.
+ *   Prompt ids lie in [2, vocab); PAD 0 ends the prompt and every entry after it must be 0; EOS 1 is not allowed.  A
+ *   violation returns MT3_ERR_BAD_ARG before any decode step runs (the check costs one kernel and an 8-byte copy back,
+ *   and synchronises the stream).
+ *   tokens_out[b, j] = prompt[b, j] for j < p_b; from p_b on the loop chooses (greedy, or MT3_GEN_BEAM1), conditioned on
+ *   the prefix.  num_steps bounds the whole row, prompt included (T5X's max_decode_len), and *steps_run counts the
+ *   prompt's positions too.
+ *   Scores follow T5X's convention for forced prompts: forced tokens are not the model's choices.  token_scores_out is 0
+ *   at forced positions; greedy's score sums the free positions; MT3_GEN_BEAM1 starts its live log-probability at 0 where
+ *   the prompt ends, makes no "prefix + EOS" hypothesis at a forced position and keeps the brevity penalty of the full
+ *   length.  A sequence cannot finish inside its prompt.
+ *   The prefix all rows share, P = min p_b, is prefilled: one teacher-forced pass (mt3_decode_teacher_forced's kernels)
+ *   writes the K/V rows of positions 0 .. P-1 into the decode cache and the loop starts at position P.  Positions from P to
+ *   p_b are forced inside the loop.  In the wgmma gemm modes the first prefill builds the pass's decoder weights.
+ *   workspace: the teacher-forced workspace, mt3_teacher_forced_workspace_bytes(m, B, T, prompt_len) bytes, 256-byte
+ *   aligned (MT3_ERR_WORKSPACE otherwise); it may be NULL only when prompt_len == 0.
+ * With prompt_len == 0, or every row empty, this is mt3_generate_scored: the same tokens and scores, bit for bit, no pass. */
+int mt3_generate_prompted(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt, int32_t prompt_len,
+                          int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+
 /* GenericTokenVocabulary._decode_tf (vocabularies.py:241-271): ids DEV i32 [B, L]
  * -> out DEV i32 [B, L] with id-3, EOS-and-after = -1, invalid = -2. */
 int mt3_vocab_decode(const int32_t* ids, int32_t batch, int32_t length, int32_t num_regular_tokens, int32_t* out,

@@ -301,19 +301,24 @@ __device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, in
 // token_scores (optional, row stride out_ld): [b, pos] = logits[next] - logsumexp(logits row) (block_logsumexp), 0 for a
 // sequence that had finished before this step (it emits PAD); NaN when the row holds a NaN.
 // y_next (optional) = E[next] + PE[pos + 1], skipped at the last step, where pos + 1 = pe_rows has no PE row.
+// plen (optional, [B]): forced prompt lengths (mt3_generate_prompted).  At pos < plen[b] the sequence emits the token the
+// caller put at tokens_out[b, pos] instead of its argmax: score 0, no finish; tok_cur and y_next follow that token.
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
                    int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
-                   int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0, const float* __restrict__ emb,
+                   const int* __restrict__ plen, int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0,
+                   const float* __restrict__ emb,
                    const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
   __shared__ float sv[8], slse[8];
   __shared__ int si[8], snan[8];
   __shared__ int s_next[2];
-  pdl_wait();
-  pdl_trigger();
   // B = sequences in the whole batch (the arrival counter spans every sub-batch), b0 = first sequence of this launch
   const int b = b0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // plen is written before the encoder runs, never by the kernel this one may start under: its load goes ahead of the wait
+  const int pl = (plen && tid == 0) ? plen[b] : 0;
+  pdl_wait();
+  pdl_trigger();
   const float* l = logits + (long long)b * V;
   // every number beats the start (-inf, 0x7fffffff), so bi stays out of range only when the whole row is NaN, and then
   // nan_i = 0 replaces it
@@ -343,7 +348,10 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
     const int pos = state[0];
     int nxt = bi;
     float lp = token_scores ? l[bi] - lse : 0.f;
-    if (finished) {
+    if (pos < pl) {                       // forced: the prompt token (never EOS), so the sequence cannot finish here
+      nxt = tokens_out[(long long)b * out_ld + pos];
+      lp = 0.f;
+    } else if (finished) {
       if (finished[b]) { nxt = 0; lp = 0.f; }
       if (nxt == 1) finished[b] = 1;
     }
@@ -389,10 +397,10 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
 
 // sequences b0 .. b0 + n_cta - 1 of a batch of B
 inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
-                              int out_ld, int* tok_out_user, int* state, int advance, int b0, const float* emb, const float* pe,
-                              int pe_rows, int D, float* y_next, int n_cta, cudaStream_t s) {
+                              int out_ld, const int* plen, int* tok_out_user, int* state, int advance, int b0, const float* emb,
+                              const float* pe, int pe_rows, int D, float* y_next, int n_cta, cudaStream_t s) {
   MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
-                               token_scores, out_ld, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
+                               token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -414,7 +422,9 @@ inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, i
 // beam_f [B][2] = {live_lp, finished score}, beam_i [B] = length of the best finished hypothesis (0 = none yet).
 // token_scores (optional, row stride out_ld): [b, pos] = the live token's log-probability v1 - lse; with it, fin_lp_eos [B]
 // keeps the EOS log-probability of the best finished hypothesis, which beam1_finalize_kernel puts at its last position.
-// y_next as in argmax_step_kernel.
+// y_next and plen as in argmax_step_kernel: at a forced position the live prefix takes the prompt token with
+// log-probability 0 (T5X's convention for prompts: forced tokens are not the model's choices), and no "prefix + EOS"
+// hypothesis is made, so the live log-probability is still 0 when the prompt ends.
 // ---------------------------------------------------------------------------------
 // Candidate order: larger value first, NaN above every number, lower id first among equals (and among NaNs).  The
 // candidates start from (-inf, 0x7fffffff), which every real candidate beats.
@@ -425,15 +435,16 @@ __device__ __forceinline__ bool cand_better(float v, int i, float ov, int oi) {
 
 __global__ void __launch_bounds__(256)
 beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
-                  int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, int* __restrict__ state,
-                  float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
+                  int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                  int* __restrict__ state, float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
                   const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
   __shared__ float s1v[8], s2v[8], smx[8], ssum[8];
   __shared__ int s1i[8], s2i[8];
   __shared__ int s_next[2];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int pl = (plen && tid == 0) ? plen[b] : 0;      // ahead of the wait, as in argmax_step_kernel
   pdl_wait();
   pdl_trigger();
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* l = logits + (long long)b * V;
   // best and second-best NON-EOS candidates (value, id), and the running maximum over everything for the log-sum-exp
   float v1 = -INFINITY, v2 = -INFINITY, mx = -INFINITY;
@@ -481,8 +492,10 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
     const int pos = state[0];
     const float live_prev = beam_f[2 * b];
     float fin_score = beam_f[2 * b + 1];
+    const bool forced = pos < pl;
+    if (forced) i1 = tokens_out[(long long)b * out_ld + pos];
     // EOS is one of the 2 best extensions iff it beats the second-best non-EOS candidate
-    if (cand_better(veos, 1, v2, i2)) {
+    if (!forced && cand_better(veos, 1, v2, i2)) {
       const float cand = (live_prev + (veos - lse)) / powf((5.0f + (float)(pos + 1)) / 6.0f, alpha);
       if (cand > fin_score) {
         fin_score = cand;
@@ -491,11 +504,11 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
         if (token_scores) fin_lp_eos[b] = veos - lse;
       }
     }
-    const float live = live_prev + (v1 - lse);
+    const float live = forced ? live_prev : live_prev + (v1 - lse);
     beam_f[2 * b] = live;
     tok_cur[b] = i1;
     tokens_out[(long long)b * out_ld + pos] = i1;
-    if (token_scores) token_scores[(long long)b * out_ld + pos] = v1 - lse;
+    if (token_scores) token_scores[(long long)b * out_ld + pos] = forced ? 0.f : v1 - lse;
     finished[b] = (beam_i[b] > 0 && fin_score > live / powf((5.0f + (float)max_len) / 6.0f, alpha)) ? 1 : 0;
     s_next[0] = i1;
     s_next[1] = pos + 1;
@@ -525,10 +538,10 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
 }
 
 inline int launch_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
-                             int out_ld, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha, int max_len,
-                             const float* emb, const float* pe, int pe_rows, int D, float* y_next, cudaStream_t s) {
+                             int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
+                             int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next, cudaStream_t s) {
   MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
-                               token_scores, out_ld, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
+                               token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }

@@ -132,6 +132,9 @@ struct Model {
   float* beam_f = nullptr; int* beam_i = nullptr;   // beam-size-1 search state (MT3_GEN_BEAM1)
   float* fin_lp_eos = nullptr;    // [B] EOS log-probability of each best finished hypothesis (beam_f's third float per sequence)
   float *tok_scores = nullptr, *seq_scores = nullptr;   // [B, L] and [B] of mt3_generate_scored
+  int* plen = nullptr;            // [B] forced prompt lengths of the token pickers (0 = free from position 0)
+  int* prompt_info = nullptr;     // {P = shortest prompt, 1 + first invalid row or 0} of prompt_scan_kernel
+  int* pf_tok = nullptr;          // [2][B, L] decoder inputs and key-validity targets of the prefill pass
   float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
   int dcounters_n = 0;
   int* dcounters = nullptr;
@@ -514,11 +517,12 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
   float* y_next = loop_step ? m->dy : nullptr;
   float* tok_scores = scored ? m->tok_scores : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
-    MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->state, m->beam_f, m->fin_lp_eos,
-                              m->beam_i, 0.6f, m->L, m->emb, m->pe, m->pe_rows, m->D, y_next, s));
+    MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->beam_f,
+                              m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, m->pe_rows, m->D, y_next, s));
   } else if (greedy) {
     MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
-                               tok_scores, m->L, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D, y_next, m->B, s));
+                               tok_scores, m->L, loop_step ? m->plen : nullptr, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D,
+                               y_next, m->B, s));
   } else {
     MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
     MT3_LAUNCH_CHECK();
@@ -674,8 +678,37 @@ static int ensure_tf_weights(Model* m, cudaStream_t s) {
   return MT3_OK;
 }
 
+// Positions t < n of every sequence of the pass's self-attention K/V -> the decode cache: head-major rows [b][K|V][h][cap] at
+// positions 0 .. n - 1, in kv_fmt, through kv_dest / kv_store (the row writer of the GEMM epilogues and the decode append).
+// K from qkv [B*Lp, 3Q] (columns Q ..); V from qkv's columns 2Q .. or, where the wgmma attention runs, from its V^T
+// [B*H*64, Lp] (keys in vt_key_slot() order).  hi + lo is the float32 value the pass attends with (split_tf32 is exact).
+__global__ void prefill_kv_kernel(const float* __restrict__ qkv_hi, const float* __restrict__ qkv_lo, const float* __restrict__ vt_hi,
+                                  const float* __restrict__ vt_lo, int Lp, int H, int kv_fmt, char* __restrict__ dst, int cap) {
+  const int t = blockIdx.x, b = blockIdx.y, Q = H * 64;
+  const long long m = (long long)b * Lp + t;
+  for (int c = 4 * threadIdx.x; c < 2 * Q; c += 4 * blockDim.x) {
+    float v[4];
+    if (c < Q || !vt_hi) {
+      const long long i = m * 3 * Q + Q + c;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = qkv_hi[i + j] + (qkv_lo ? qkv_lo[i + j] : 0.f);
+    } else {
+      const int h = (c - Q) >> 6, d = (c - Q) & 63;
+      const long long i = (((long long)b * H + h) * 64 + d) * Lp + vt_key_slot(t);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = vt_hi[i + (long long)j * Lp] + (vt_lo ? vt_lo[i + (long long)j * Lp] : 0.f);
+    }
+    int d;
+    char* row = dst + kv_dest(b, c, 1, cap, H, t, kv_fmt, d);
+    kv_store<4>(row, kv_fmt, d, v);
+  }
+}
+
+// kv_cache: the prefill form (mt3_generate_prompted).  Every layer's self-attention K/V of positions 0 .. L - 1 go to the
+// decode cache (kv_layer(m, kv_cache, l, m->L)); nothing after the last layer's QKV projection runs, and logits and scores
+// are not computed.
 static int teacher_forced_impl(Model* m, const float* encoded, int B, int T, const int* tok_in, const int* tgt, const int* wts, int L,
-                               float* logits, float* scores, char* ws, cudaStream_t s) {
+                               float* logits, float* scores, char* ws, cudaStream_t s, char* kv_cache = nullptr) {
   const int Lp = tf_pad(L), D = m->D, Q = m->Q, F = m->F, V = m->V, H = m->H;
   const int M = B * Lp, Me = B * T;
   const bool s3 = m->split3, tcs = tc_attention(m, Lp, Lp, true), tcc = tc_attention(m, Lp, T, false);
@@ -701,6 +734,12 @@ static int teacher_forced_impl(Model* m, const float* encoded, int B, int T, con
     // self-attention: RMSNorm folded into the QKV projection's row scale; mask make_decoder_mask(targets)
     MT3_TRY(seq_rstd(m, y, M, rstd, s));
     MT3_TRY(seq_qkv(m, y, M, rstd, dl.wqkv, dl.t_wqkv, qkv, tcs ? &vt : nullptr, Lp, s));
+    if (kv_cache) {
+      prefill_kv_kernel<<<dim3(L, B), 128, 0, s>>>(qkv.hi, qkv.lo, tcs ? vt.hi : nullptr, tcs ? vt.lo : nullptr, Lp, H, m->kv_fmt,
+                                                   kv_layer(m, kv_cache, l, m->L), m->L);
+      MT3_LAUNCH_CHECK();
+      if (l == m->Ld - 1) return MT3_OK;
+    }
     MT3_TRY(seq_self_attention(m, qkv, tcs ? &vt : nullptr, B, Lp, tgt, L, true, ao, scratch, s));
     MT3_TRY(seq_residual(m, y, M, ao, Q, dl.wo, dl.t_wo, s));
     // cross-attention over all T encoder positions; K/V projected from `encoded` for this layer
@@ -937,7 +976,7 @@ struct WsLayout {
   int64_t x_hi, x_lo, h_lo, ao_lo, g_lo, enc_hi, enc_lo, qkv_lo, vt_hi, vt_lo;
   int64_t dy2, dssq;
   int64_t h, rstd, qkv, ao, g, encoded, ckv, skv, dy, drstd, dq, dao, dg, dlogits, tok_cur, finished, tokens, state, dpartial, dcounters, beam_f, beam_i, att_scratch;
-  int64_t tok_scores, seq_scores, total;
+  int64_t tok_scores, seq_scores, plen, prompt_info, pf_tok, total;
 };
 WsLayout ws_layout(const Model* m, int B, int T) {
   WsLayout w;
@@ -982,6 +1021,9 @@ WsLayout ws_layout(const Model* m, int B, int T) {
   w.beam_i = take((int64_t)B * 4);
   w.tok_scores = take((int64_t)B * L * 4);
   w.seq_scores = take((int64_t)B * 4);
+  w.plen = take((int64_t)B * 4);
+  w.prompt_info = take(2 * 4);
+  w.pf_tok = take((int64_t)2 * B * L * 4);
   w.total = off;
   return w;
 }
@@ -1013,6 +1055,7 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
   m->dpartial = (float*)(b + w.dpartial); m->dcounters = (int*)(b + w.dcounters);
   m->beam_f = (float*)(b + w.beam_f); m->beam_i = (int*)(b + w.beam_i); m->fin_lp_eos = m->beam_f + 2 * batch;
   m->tok_scores = (float*)(b + w.tok_scores); m->seq_scores = (float*)(b + w.seq_scores);
+  m->plen = (int*)(b + w.plen); m->prompt_info = (int*)(b + w.prompt_info); m->pf_tok = (int*)(b + w.pf_tok);
   const bool key_split = m->tc && attention_tc_scratch_floats(batch, input_length, input_length, m->H, false) > 0;
   m->att_scratch = key_split ? (float*)(b + w.att_scratch) : nullptr;
   m->dcounters_n = cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN);
@@ -1059,9 +1102,71 @@ extern "C" int mt3_decode_step(mt3_model* h, const int32_t* tok_in, float* logit
                           (cudaStream_t)stream);
 }
 
-// mt3_generate and mt3_generate_scored; `name` is the entry point the caller used, for its error messages
-static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
-                         float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream) {
+// Prompt rows [B, prompt_len] (mt3_generate_prompted), one warp per row: p_b = the length of the non-zero prefix,
+// which must hold ids in [2, V), with only 0 after it.  Writes plen[b] = p_b and the row into tokens[b, 0 .. prompt_len);
+// info = {min p_b, 1 + the first invalid row (0 when every row is valid)}.
+__global__ void __launch_bounds__(256) prompt_scan_kernel(const int* __restrict__ prompt, int B, int prompt_len, int V,
+                                                          int* __restrict__ plen, int* __restrict__ tokens, int ld_tokens,
+                                                          int* __restrict__ info) {
+  __shared__ int s_min, s_bad;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) { s_min = prompt_len; s_bad = B; }
+  __syncthreads();
+  for (int b = warp; b < B; b += 8) {
+    const int* row = prompt + (long long)b * prompt_len;
+    int p = prompt_len;
+    for (int j0 = 0; j0 < prompt_len; j0 += 32) {
+      const int j = j0 + lane;
+      const unsigned z = __ballot_sync(0xffffffffu, j < prompt_len && row[j] == 0);
+      if (z) { p = j0 + __ffs(z) - 1; break; }
+    }
+    bool bad = false;
+    for (int j = lane; j < prompt_len; j += 32) {
+      const int v = row[j];
+      bad |= j < p ? (v < 2 || v >= V) : v != 0;
+      tokens[(long long)b * ld_tokens + j] = v;
+    }
+    if (lane == 0) plen[b] = p;
+    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicMin(&s_bad, b);
+    if (lane == 0) atomicMin(&s_min, p);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) { info[0] = s_min; info[1] = s_bad < B ? s_bad + 1 : 0; }
+}
+
+// The prefill pass's inputs over the shared prefix of P positions: decoder inputs BOS, prompt[:, 0 .. P-2] and targets
+// prompt[:, 0 .. P-1] (all non-zero: every key < P is valid), both [B, P]; and the loop's state after it: position P, next
+// decoder input prompt[:, P-1].
+__global__ void prefill_inputs_kernel(const int* __restrict__ prompt, int prompt_len, int P, int* __restrict__ dec_in,
+                                      int* __restrict__ tgt, int* __restrict__ tok_cur, int* __restrict__ state) {
+  const int b = blockIdx.x;
+  const int* row = prompt + (long long)b * prompt_len;
+  for (int j = threadIdx.x; j < P; j += blockDim.x) {
+    dec_in[(long long)b * P + j] = j ? row[j - 1] : 0;
+    tgt[(long long)b * P + j] = row[j];
+  }
+  if (threadIdx.x == 0) {
+    tok_cur[b] = row[P - 1];
+    if (b == 0) state[0] = P;
+  }
+}
+
+// Shortest shared prompt prefix worth one teacher-forced pass instead of stepping the loop through it.  Measured at bench's
+// configuration (DESIGN.md §6): the pass over P <= 128 positions costs about as much as the loop's first 17 steps.
+constexpr int kPrefillMinP = 20;
+
+// Whether the teacher-forced pass can prefill P positions: the exact-fp32 attention kernel's limits where it runs
+static bool prefill_supported(const Model* m, int P) {
+  const int Lp = tf_pad(P);
+  return (tc_attention(m, Lp, Lp, true) || attention_fp32_smem(Lp) <= kAttFp32MaxSmem) &&
+         (tc_attention(m, Lp, m->T, false) || attention_fp32_smem(m->T) <= kAttFp32MaxSmem);
+}
+
+// mt3_generate, mt3_generate_scored and mt3_generate_prompted; `name` is the entry point the caller used, for its error
+// messages.  prompt_len == 0: no prompt (prompt and workspace unused).
+static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
+                         int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run,
+                         void* workspace, int64_t workspace_bytes, void* stream) {
   MT3_REQUIRE(h && x && tokens_out, MT3_ERR_BAD_ARG, "%s: null argument", name);
   Model* m = reinterpret_cast<Model*>(h);
   MT3_NEED_WS(m);
@@ -1069,10 +1174,33 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
               m->L);
   MT3_REQUIRE((flags & ~(MT3_GEN_STOP_AT_EOS | MT3_GEN_USE_GRAPH | MT3_GEN_BEAM1)) == 0, MT3_ERR_BAD_ARG, "%s: unknown flag bits 0x%x", name,
               flags);
+  MT3_REQUIRE(prompt_len >= 0 && prompt_len <= num_steps, MT3_ERR_BAD_ARG, "%s: prompt_len %d outside [0, num_steps=%d]", name, prompt_len,
+              num_steps);
+  MT3_REQUIRE(prompt_len == 0 || prompt, MT3_ERR_BAD_ARG, "%s: prompt is NULL with prompt_len %d", name, prompt_len);
+  if (prompt_len > 0) {
+    MT3_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, MT3_ERR_WORKSPACE,
+                "%s: the teacher-forced workspace must be non-null and 256-byte aligned when prompt_len > 0", name);
+    const int64_t need = tf_layout(m, m->B, m->T, prompt_len).total;
+    MT3_REQUIRE(workspace_bytes >= need, MT3_ERR_WORKSPACE, "%s: workspace has %lld bytes, %lld needed", name, (long long)workspace_bytes,
+                (long long)need);
+  }
   cudaStream_t s = (cudaStream_t)stream;
+  MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
+  MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
+  int P = 0;                                    // prompt prefix every row shares
+  if (prompt_len > 0) {
+    prompt_scan_kernel<<<1, 256, 0, s>>>(prompt, m->B, prompt_len, m->V, m->plen, m->tokens, m->L, m->prompt_info);
+    MT3_LAUNCH_CHECK();
+    MT3_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 2, m->prompt_info, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    MT3_CUDA_CHECK(cudaStreamSynchronize(s));
+    if (m->h_flag[3]) {
+      MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
+      return fail(MT3_ERR_BAD_ARG, "%s: prompt row %d is not a prefix of ids in [2, %d) followed by zeros", name, m->h_flag[3] - 1, m->V);
+    }
+    P = m->h_flag[2];
+  }
   MT3_TRY(encode_impl(m, x, m->encoded, s));
   MT3_TRY(cross_kv_impl(m, m->encoded, s));
-  MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
   const bool scored = token_scores_out || scores_out;
   if (scored) MT3_CUDA_CHECK(cudaMemsetAsync(m->tok_scores, 0, (size_t)m->B * m->L * sizeof(float), s));
   const bool use_graph = (flags & MT3_GEN_USE_GRAPH) != 0;
@@ -1085,23 +1213,37 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
     MT3_CUDA_CHECK(cudaStreamSynchronize(s));        // `init` is stack-owned pageable memory
     MT3_CUDA_CHECK(cudaMemsetAsync(m->beam_i, 0, (size_t)m->B * sizeof(int), s));
   }
+  // the shared prefix: one teacher-forced pass writes its K/V rows into the cache, and the loop starts at position P.
+  // The tokens there are forced (plen), so they score 0 and finish nothing, as the loop's forced steps do.
+  int start = 0;
+  if (P >= kPrefillMinP && prefill_supported(m, P)) {
+    MT3_REQUIRE(tf_layout(m, m->B, m->T, P).total <= workspace_bytes, MT3_ERR_WORKSPACE, "%s: workspace too small for the prefill", name);
+    MT3_TRY(ensure_tf_weights(m, s));
+    int* dec_in = m->pf_tok;
+    int* tgt = m->pf_tok + (int64_t)m->B * P;
+    prefill_inputs_kernel<<<m->B, 128, 0, s>>>(prompt, prompt_len, P, dec_in, tgt, m->tok_cur, m->state);
+    MT3_LAUNCH_CHECK();
+    MT3_TRY(teacher_forced_impl(m, m->encoded, m->B, m->T, dec_in, tgt, nullptr, P, nullptr, nullptr, (char*)workspace, s, m->skv));
+    start = P;
+    m->host_pos = P;
+  }
   constexpr int kBlock = 16;                    // steps per graph launch (and between two polls of the all-finished flag)
   cudaGraphExec_t g1 = nullptr, gN = nullptr;
   uint64_t k1 = 0, kN = 0;
   if (use_graph) {
-    if (num_steps >= kBlock) {
+    if (num_steps - start >= kBlock) {
       MT3_TRY(ensure_graph(m, mode, kBlock, scored));
       gN = m->graph_exec; kN = m->graph_kernels;
     }
-    if (num_steps % kBlock != 0) {
+    if ((num_steps - start) % kBlock != 0) {
       MT3_TRY(ensure_graph(m, mode, 1, scored));
       g1 = m->graph_exec; k1 = m->graph_kernels;
     }
   }
-  if (num_steps > 0)       // decoder input of step 0: BOS (tok_cur was zeroed by cross_kv) at position 0; later ones come from the argmax kernel
-    MT3_TRY(dec_embed(m, m->tok_cur, s));
-  int ran = 0;
-  for (int step = 0; step < num_steps;) {
+  if (num_steps > start)   // decoder input of the first step: BOS (tok_cur was zeroed by cross_kv) at position 0, or the prompt's
+    MT3_TRY(dec_embed(m, m->tok_cur, s));      // token P - 1 at position P; later ones come from the token picker
+  int ran = start;
+  for (int step = start; step < num_steps;) {
     int n = 1;
     if (use_graph && gN && num_steps - step >= kBlock) {
       MT3_CUDA_CHECK(cudaGraphLaunch(gN, s));
@@ -1116,7 +1258,7 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
     step += n;
     ran += n;
     m->host_pos += n;
-    if (stop && ((step & 15) == 0 || step == num_steps)) {
+    if (stop && (((step - start) & 15) == 0 || step == num_steps)) {
       MT3_CUDA_CHECK(cudaMemcpyAsync(m->h_flag, m->state + 2, sizeof(int), cudaMemcpyDeviceToHost, s));
       MT3_CUDA_CHECK(cudaStreamSynchronize(s));
       if (m->h_flag[0]) break;
@@ -1138,12 +1280,20 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
 
 extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                             int32_t* steps_run, void* stream) {
-  return generate_impl("mt3_generate", h, x, num_steps, flags, tokens_out, nullptr, nullptr, steps_run, stream);
+  return generate_impl("mt3_generate", h, x, num_steps, flags, nullptr, 0, tokens_out, nullptr, nullptr, steps_run, nullptr, 0, stream);
 }
 
 extern "C" int mt3_generate_scored(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                                    float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream) {
-  return generate_impl("mt3_generate_scored", h, x, num_steps, flags, tokens_out, token_scores_out, scores_out, steps_run, stream);
+  return generate_impl("mt3_generate_scored", h, x, num_steps, flags, nullptr, 0, tokens_out, token_scores_out, scores_out, steps_run,
+                       nullptr, 0, stream);
+}
+
+extern "C" int mt3_generate_prompted(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
+                                     int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out,
+                                     int32_t* steps_run, void* workspace, int64_t workspace_bytes, void* stream) {
+  return generate_impl("mt3_generate_prompted", h, x, num_steps, flags, prompt, prompt_len, tokens_out, token_scores_out, scores_out,
+                       steps_run, workspace, workspace_bytes, stream);
 }
 
 extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length, int32_t target_length) {

@@ -165,15 +165,15 @@ KH_API int kh_p24_roundtrip(const float* x, float* y, uint32_t* code, long long 
 KH_API int kh_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* tok_user,
                           int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows, int D, float* y_next,
                           int n_cta) {
-  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, tok_user, state, advance, b0, emb, pe, pe_rows,
-                            D, y_next, n_cta, 0);
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, nullptr, tok_user, state, advance, b0, emb, pe,
+                            pe_rows, D, y_next, n_cta, 0);
 }
 
 KH_API int kh_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
                          float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
                          float* y_next) {
-  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, state, beam_f, nullptr, beam_i, alpha, max_len,
-                           emb, pe, pe_rows, D, y_next, 0);
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, nullptr, state, beam_f, nullptr, beam_i, alpha,
+                           max_len, emb, pe, pe_rows, D, y_next, 0);
 }
 
 KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i) {
@@ -185,15 +185,31 @@ KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* be
 KH_API int kh_argmax_step_scored(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                                  int out_ld, int* tok_user, int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows,
                                  int D, float* y_next, int n_cta) {
-  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, tok_user, state, advance, b0, emb, pe,
-                            pe_rows, D, y_next, n_cta, 0);
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, nullptr, tok_user, state, advance, b0, emb,
+                            pe, pe_rows, D, y_next, n_cta, 0);
 }
 
 KH_API int kh_beam1_step_scored(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                                 int out_ld, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha, int max_len,
                                 const float* emb, const float* pe, int pe_rows, int D, float* y_next) {
-  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, state, beam_f, fin_lp_eos, beam_i, alpha,
-                           max_len, emb, pe, pe_rows, D, y_next, 0);
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, nullptr, state, beam_f, fin_lp_eos, beam_i,
+                           alpha, max_len, emb, pe, pe_rows, D, y_next, 0);
+}
+
+// The forced forms (mt3_generate_prompted): plen [B] prompt lengths; at pos < plen[b] the kernels emit tokens_out[b, pos]
+// (which the caller fills) with score 0 and no finish.  token_scores (and fin_lp_eos) may be NULL.
+KH_API int kh_argmax_step_forced(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                 int out_ld, const int* plen, int* tok_user, int* state, int advance, int b0, const float* emb,
+                                 const float* pe, int pe_rows, int D, float* y_next, int n_cta) {
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, tok_user, state, advance, b0, emb, pe,
+                            pe_rows, D, y_next, n_cta, 0);
+}
+
+KH_API int kh_beam1_step_forced(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
+                                int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next) {
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i,
+                           alpha, max_len, emb, pe, pe_rows, D, y_next, 0);
 }
 
 KH_API int kh_beam1_finalize_scored(int* tokens, int B, int L, int steps, const int* beam_i, float* token_scores, const float* beam_f,

@@ -167,12 +167,14 @@ class InferenceModel(object):
         return self.vocabulary.decode_tf(prediction).cpu().numpy()
 
     def transcribe_segments(self, audio_segments, n_valid_frames=None, num_steps: Optional[int] = None,
-                            stop_at_eos: bool = True, decoded: bool = True, return_scores: bool = False):
+                            stop_at_eos: bool = True, decoded: bool = True, return_scores: bool = False, prompts=None):
         """Hot path end to end for already-cut segments: host float32 [S, inputs_length*hop] ->
         host int32 [S, 1024].  H2D copy, log-mel kernel, encoder, greedy decoder, (vocab decode),
         D2H copy; batches of `batch_size`.  This is the call bench.py's `e2e` times.
         return_scores=True returns (tokens, token_scores float32 [S, 1024], scores float32 [S]) with the same tokens: how sure
-        the model was of each emitted token (its log-probability; 0 after EOS) and of each segment (Transformer.generate)."""
+        the model was of each emitted token (its log-probability; 0 after EOS) and of each segment (Transformer.generate).
+        prompts: host int [S, P], a forced start per segment (Transformer.generate's `prompt`), e.g. the tie section of
+        segment_score_targets' decoder_target_tokens: the output rows start with them and decode on from there."""
         a = audio_segments
         if isinstance(a, np.ndarray):
             a = torch.from_numpy(a)
@@ -180,6 +182,10 @@ class InferenceModel(object):
         if not a.is_cuda and not a.is_pinned():
             a = a.pin_memory()              # so that the per-batch H2D copies below are truly asynchronous
         S = a.shape[0]
+        if prompts is not None:
+            prompts = np.asarray(prompts)
+            if prompts.ndim != 2 or prompts.shape[0] != S:
+                raise ValueError('prompts must be [S=%d, P]; got shape %s' % (S, prompts.shape))
         out = torch.empty((S, self.outputs_length), dtype=torch.int32, pin_memory=True)
         if return_scores:
             out_ts = torch.empty((S, self.outputs_length), dtype=torch.float32, pin_memory=True)
@@ -194,7 +200,8 @@ class InferenceModel(object):
                                                     n_valid_frames=None if nv is None else nv[s0:s1])
             spec = self._pad_inputs(spec)
             toks = self.model.generate(spec, num_steps=num_steps, stop_at_eos=stop_at_eos, use_graph=self.use_graph,
-                                       decode=self.decode, return_scores=return_scores)
+                                       decode=self.decode, return_scores=return_scores,
+                                       prompt=None if prompts is None else prompts[s0:s1])
             if return_scores:
                 toks, ts, sc = toks
                 out_ts[s0:s1].copy_(ts, non_blocking=True)
@@ -212,6 +219,8 @@ class InferenceModel(object):
         list, transcribes its contiguous shard on its own GPU and receives all token streams
         int32 [S, 1024] in segment order after ONE all-gather (three with return_scores=True: tokens, token scores
         and scores, as transcribe_segments returns them).  Identity with a single process."""
+        if kwargs.get('prompts') is not None:
+            raise ValueError('transcribe_segments_sharded does not take prompts; call transcribe_segments on each rank\'s segments')
         from . import distributed as mt3_dist
         rank, world_size = mt3_dist.world()
         a = audio_segments

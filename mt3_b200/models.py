@@ -105,20 +105,32 @@ class ContinuousInputsEncoderDecoderModel:
         return x
 
     def predict_batch_with_aux(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None, num_decodes: int = 1,
-                               return_all_decodes: bool = False):
+                               return_all_decodes: bool = False, prompt_with_targets: bool = False):
         """tokens int32 [B, max_decode_length] (0 after EOS) and T5X's aux dict {'scores': float32 [B]}: the greedy sequence's
         summed token log-probabilities, or beam_search's length-normalised score.  A module whose `generate` cannot return
         scores (no `return_scores` argument) gives an empty aux dict.  return_all_decodes=True adds T5X's decodes axis:
         tokens [B, 1, max_decode_length], scores [B, 1].  `params` is accepted for signature fidelity: the weights live in
-        the module."""
+        the module.
+        prompt_with_targets=True (T5X): batch['decoder_input_tokens'][:, 1:] is the prompt -- each row's non-zero prefix is
+        forced and returned inside the decodes (Transformer.generate's `prompt`).  Column 0 is the BOS 0 of the
+        right-shifted targets."""
         del params, rng
         x = self._inputs(batch, decoder_params, num_decodes)
+        kw = {}
+        if prompt_with_targets:
+            din = np.asarray(batch['decoder_input_tokens'].cpu() if hasattr(batch['decoder_input_tokens'], 'cpu')
+                             else batch['decoder_input_tokens'])
+            if din.ndim != 2 or din.shape[1] < 1:
+                raise ValueError('decoder_input_tokens must be [batch, length >= 1]; got shape %s' % (din.shape,))
+            if (din[:, 0] != 0).any():
+                raise ValueError('decoder_input_tokens[:, 0] must be BOS 0 (the targets shifted right)')
+            kw['prompt'] = np.ascontiguousarray(din[:, 1:])
         aux = {}
         if 'return_scores' in inspect.signature(self.module.generate).parameters:
-            tokens, _, scores = self.module.generate(x, stop_at_eos=True, decode=self._decode, return_scores=True)
+            tokens, _, scores = self.module.generate(x, stop_at_eos=True, decode=self._decode, return_scores=True, **kw)
             aux['scores'] = scores[:, None] if return_all_decodes else scores
         else:
-            tokens = self.module.generate(x, stop_at_eos=True, decode=self._decode)
+            tokens = self.module.generate(x, stop_at_eos=True, decode=self._decode, **kw)
         return (tokens[:, None] if return_all_decodes else tokens), aux
 
     def predict_batch(self, params, batch: Mapping[str, Any], rng=None, decoder_params=None):

@@ -242,25 +242,34 @@ class Transformer:
         return torch.cat(outs, dim=1)
 
     def generate(self, encoder_input_tokens: torch.Tensor, num_steps: Optional[int] = None, stop_at_eos: bool = True,
-                 use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy', return_scores: bool = False):
+                 use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy', return_scores: bool = False,
+                 prompt=None):
         """encode + decode from BOS=0 (models.py:121-138).  decode='greedy': argmax until EOS; decode='beam1': T5X's
         decoding.beam_search at num_decodes=1, the reference's decode_fn (models.py:127) -- they differ when EOS is one of the
         two best tokens without being decisive (tests/test_beam1.py).  Returns raw model ids int32 [B, max_decode_length],
         0 after EOS.
         return_scores=True returns (tokens, token_scores float32 [B, max_decode_length], scores float32 [B]) with the same
         tokens: each emitted token's log-probability (0 after EOS and beyond the steps run) and the sequence score -- greedy,
-        the sum of the token scores; beam1, T5X beam_search's length-normalised score (mt3_generate_scored)."""
+        the sum of the token scores; beam1, T5X beam_search's length-normalised score (mt3_generate_scored).
+        prompt: int [B, P] (torch or numpy), T5X's prompt_with_targets: row b's non-zero prefix is forced -- the output row
+        starts with it, its positions score 0, and the loop chooses from its end on.  Ids in [2, vocab_size), 0 after the
+        prefix, no EOS, P <= num_steps (mt3_generate_prompted).  The prefix every row shares is prefilled by one
+        teacher-forced pass."""
         if decode not in ('greedy', 'beam1'):
             raise ValueError("decode must be 'greedy' or 'beam1'")
         x = self._check_inputs(encoder_input_tokens)
         b, t, _ = x.shape
-        self._bind(b, t)
         steps = self.max_decode_length if num_steps is None else int(num_steps)
+        if prompt is not None:
+            prompt = self._check_prompt(prompt, b, steps)
+        self._bind(b, t)
         if out is None:
             out = torch.empty((b, self.max_decode_length), dtype=torch.int32, device=self.device)
         flags = (_lib.GEN_STOP_AT_EOS if stop_at_eos else 0) | (_lib.GEN_USE_GRAPH if use_graph else 0) | \
                 (_lib.GEN_BEAM1 if decode == 'beam1' else 0)
         ran = C.c_int32(0)
+        if prompt is not None and prompt.shape[1] > 0:
+            return self._generate_prompted(x, steps, flags, prompt, out, return_scores)
         if not return_scores:
             with torch.cuda.device(self.device):
                 _lib.check(self._lib.mt3_generate(self._h, x.data_ptr(), steps, flags, out.data_ptr(), C.byref(ran), self._stream()))
@@ -273,3 +282,41 @@ class Transformer:
                                                      scores.data_ptr(), C.byref(ran), self._stream()))
         self.last_steps_run = int(ran.value)
         return out, token_scores, scores
+
+    def _check_prompt(self, prompt, batch: int, num_steps: int) -> torch.Tensor:
+        """The host-side check of a generate prompt (the library checks it again on the device): int32 [B, P] on the device."""
+        p = self._tokens(prompt, 'prompt')
+        if p.shape[0] != batch:
+            raise ValueError(f'prompt has batch {p.shape[0]}, the inputs have {batch}')
+        if p.shape[1] > num_steps:
+            raise ValueError(f'prompt length {p.shape[1]} exceeds num_steps={num_steps} (the steps include the prompt)')
+        if p.numel():
+            v = self.config.vocab_size
+            lo, hi = int(p.min()), int(p.max())
+            if lo < 0 or hi >= v:
+                raise ValueError(f'prompt: ids must lie in [0, vocab_size={v}); got [{lo}, {hi}]')
+            if bool((p == 1).any()):
+                raise ValueError('prompt: EOS (1) is not allowed inside a prompt')
+            ended = torch.cumsum((p == 0).to(torch.int32), dim=1) > 0
+            if bool((ended & (p != 0)).any()):
+                raise ValueError('prompt: a row has non-zero ids after its first 0 (PAD ends the prompt)')
+        return p
+
+    def _generate_prompted(self, x, steps: int, flags: int, prompt: torch.Tensor, out: torch.Tensor, return_scores: bool):
+        b, t, _ = x.shape
+        nbytes = int(self._lib.mt3_teacher_forced_workspace_bytes(self._h, b, t, prompt.shape[1]))
+        if nbytes <= 0:
+            raise _lib.Mt3Error(-2, f"no teacher-forced workspace layout for batch={b}, input_length={t}, length={prompt.shape[1]}")
+        if self._tf_ws is None or self._tf_ws.numel() < nbytes:
+            self._tf_ws = None
+            self._tf_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        token_scores = torch.empty((b, self.max_decode_length), dtype=torch.float32, device=self.device) if return_scores else None
+        scores = torch.empty((b,), dtype=torch.float32, device=self.device) if return_scores else None
+        ran = C.c_int32(0)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.mt3_generate_prompted(
+                self._h, x.data_ptr(), steps, flags, prompt.data_ptr(), prompt.shape[1], out.data_ptr(),
+                None if token_scores is None else token_scores.data_ptr(), None if scores is None else scores.data_ptr(), C.byref(ran),
+                self._tf_ws.data_ptr(), self._tf_ws.numel(), self._stream()))
+        self.last_steps_run = int(ran.value)
+        return (out, token_scores, scores) if return_scores else out
