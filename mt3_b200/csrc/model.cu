@@ -77,22 +77,68 @@ struct TcW { float* hi = nullptr; float* lo = nullptr; TcOperand op; int K = 0, 
 // An activation buffer [rows, ld]; lo != null when it is carried as a tf32 hi/lo pair.
 struct Act { float* hi = nullptr; float* lo = nullptr; TcOperand op; };
 
+// A bump allocator over one device region, in steps of `align` bytes (256 in the workspaces, one float in the weight slabs).
+// base == nullptr only measures: take() returns null and `used` grows all the same, so the one function that carves a
+// region also states its size.  take(0) is null and takes nothing.
+struct Carve {
+  char* base = nullptr;
+  int64_t align = 256;
+  int64_t used = 0;
+  template <class T = float> T* take(int64_t n) {
+    if (n <= 0) return nullptr;
+    T* r = base ? (T*)(base + used) : nullptr;
+    used += align_up(n * (int64_t)sizeof(T), align);
+    return r;
+  }
+};
+
+// What the full-sequence layer steps (seq_*) work on, for B sequences of T rows: the residual stream h, its RMSNorm
+// statistic, qkv, the attention output ao and the MLP hidden g (lo planes in TF32X3).  Where the self-attention runs on
+// the wgmma kernel (tc_attn), qkv also has its lo plane, V^T [B*H*64, T] exists and so does the key-split scratch;
+// elsewhere no kernel reads them.  The encoder carves one set in the model workspace, the teacher-forced pass one in its own.
+struct SeqActs {
+  int B = 0, T = 0;
+  bool tc_attn = false;
+  Act h, qkv, vt, ao, g;
+  float* rstd = nullptr;
+  float* scratch = nullptr;
+};
+
 struct EncLayer { float *wqkv, *wo, *wi, *wo2; TcW t_wqkv, t_wo, t_wi, t_wo2; };
 struct DecLayer {
   float *wqkv, *wo, *wq_c, *wkv_c, *wo_c, *wi, *wo2; float* wc1 = nullptr; TcW t_wkv_c;   // wc1: [Q+D, Q] = [Wo.Wq ; Wq]
   TcW t_wqkv, t_wo, t_wq_c, t_wo_c, t_wi, t_wo2;   // teacher-forced pass only: built on its first call (ensure_tf_weights)
 };
 
-struct Model {
+// The buffers of the caller's model workspace, carved by carve_workspace
+struct WsBuffers {
+  SeqActs ea;                     // the encoder's activations
+  Act a_x, a_enc;                 // TF32X3 only: hi/lo splits of the caller's encoder input and of `encoded`
+  float* encoded = nullptr;
+  char *ckv = nullptr, *skv = nullptr;   // head-major K/V rows (kv_row bytes each)
+  float *dy = nullptr, *dy2 = nullptr;   // the decode step's residual stream and its ping-pong partner (dec_layer_outq)
+  float* dssq = nullptr;          // [B][D/32] sum-of-squares partials
+  float *dq = nullptr, *dao = nullptr, *dg = nullptr, *dlogits = nullptr;
+  int *tok_cur = nullptr, *finished = nullptr, *tokens = nullptr, *state = nullptr;
+  float* beam_f = nullptr; int* beam_i = nullptr;   // beam-size-1 search state (MT3_GEN_BEAM1)
+  float* fin_lp_eos = nullptr;    // [B] EOS log-probability of each best finished hypothesis (beam_f's third float per sequence)
+  float *tok_scores = nullptr, *seq_scores = nullptr;   // [B, L] and [B] of mt3_generate_scored
+  int* plen = nullptr;            // [B] forced prompt lengths of the token pickers (0 = free from position 0)
+  int* prompt_info = nullptr;     // {P = shortest prompt, 1 + first invalid row or 0} of prompt_scan_kernel
+  int* pf_tok = nullptr;          // [2][B, L] decoder inputs and key-validity targets of the prefill pass
+  float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
+  int* dcounters = nullptr;       // [dec_tiles()]
+};
+
+constexpr int kPeRows = 2048;     // rows of the sinusoid table (FixedEmbed.max_length, layers.py:565)
+
+struct Model : WsBuffers {
   mt3_model_config cfg;
   int D, H, Q, F, V, Le, Ld, L;
   float* slab = nullptr;          // all prepared weights
   float* slab_tc = nullptr;       // K-major (and hi/lo) copies for the wgmma path
-  float *dy2 = nullptr, *dssq = nullptr;   // second residual-stream buffer (ping-pong) and [B][D/32] sum-of-squares partials
   bool tc = false, split3 = false;
   TcW t_w_in;
-  Act a_h, a_ao, a_g, a_qkv;      // encoder activations (workspace), in every mode; lo planes in TF32X3 mode only
-  Act a_x, a_enc, a_vt;           // wgmma path only: TF32X3 splits of the caller's encoder input and of `encoded`; per-head V^T
   bool pdl_attn = true;           // programmatic dependent launch of the decode attention kernels (K/V streamed under the
                                   // preceding GEMM); MT3_PDL=0 turns it off, the reference for the value-neutrality tests
   int pf_attn = 16;               // MT3_PF_ATTN=n: the decode-step attention kernels prefetch the n K/V tiles that follow their
@@ -117,27 +163,11 @@ struct Model {
   float* w_logits = nullptr;
   TcW t_w_logits;                 // teacher-forced pass only, like DecLayer::t_wqkv ...
   float* slab_tf = nullptr;       // K-major (and hi/lo) decoder weights of the teacher-forced pass; null until its first call
-  float* pe = nullptr;            // [pe_rows, D] sinusoid table (FixedEmbed.max_length, layers.py:565)
-  int pe_rows = 2048;
+  float* pe = nullptr;            // [kPeRows, D] sinusoid table
 
-  // workspace (caller-owned)
+  // workspace (caller-owned; its buffers are the WsBuffers)
   char* ws = nullptr;
-  int64_t ws_bytes = 0;
   int B = 0, T = 0;
-  float *h = nullptr, *rstd = nullptr, *qkv = nullptr, *ao = nullptr, *g = nullptr, *encoded = nullptr;
-  char *ckv = nullptr, *skv = nullptr;   // head-major K/V rows (kv_row bytes each)
-  float *dy = nullptr, *drstd = nullptr, *dq = nullptr, *dao = nullptr, *dg = nullptr, *dlogits = nullptr;
-  int *tok_cur = nullptr, *finished = nullptr, *tokens = nullptr, *state = nullptr;
-  float* att_scratch = nullptr;   // key-split encoder attention (T > 256): unnormalised O parts + (max, sum) pairs
-  float* beam_f = nullptr; int* beam_i = nullptr;   // beam-size-1 search state (MT3_GEN_BEAM1)
-  float* fin_lp_eos = nullptr;    // [B] EOS log-probability of each best finished hypothesis (beam_f's third float per sequence)
-  float *tok_scores = nullptr, *seq_scores = nullptr;   // [B, L] and [B] of mt3_generate_scored
-  int* plen = nullptr;            // [B] forced prompt lengths of the token pickers (0 = free from position 0)
-  int* prompt_info = nullptr;     // {P = shortest prompt, 1 + first invalid row or 0} of prompt_scan_kernel
-  int* pf_tok = nullptr;          // [2][B, L] decoder inputs and key-validity targets of the prefill pass
-  float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
-  int dcounters_n = 0;
-  int* dcounters = nullptr;
   bool have_cross = false;
   int host_pos = 0;               // host mirror of the device position (cache overflow guard)
 
@@ -156,19 +186,6 @@ struct Model {
 // byte address of layer l's K/V block: [B][K|V][H][cap] rows of kv_row bytes
 static char* kv_layer(const Model* m, char* base, int l, int cap) {
   return base + (int64_t)l * m->B * cap * 2 * m->H * m->kv_row;
-}
-
-static int64_t prepared_floats(const mt3_model_config& c) {
-  const int64_t D = c.emb_dim, Q = (int64_t)c.num_heads * c.head_dim, F = c.mlp_dim, V = c.vocab_size;
-  int64_t n = (int64_t)c.input_depth * D;
-  n += (int64_t)c.num_encoder_layers * (D * 3 * Q + Q * D + D * 2 * F + F * D);
-  n += D;          // encoder_norm
-  n += V * D;      // embedding
-  n += (int64_t)c.num_decoder_layers * (D * 3 * Q + Q * D + D * Q + D * 2 * Q + Q * D + D * 2 * F + F * D);
-  n += D * V;      // logits
-  n += (int64_t)c.num_decoder_layers * (Q + D) * Q;   // precomposed [Wo.Wq ; Wq] blocks
-  n += 2048 * D;   // PE
-  return n;
 }
 
 // out [Q + D, Q]: rows [0, Q) = Wo [Q, D] . Wq [D, Q] accumulated in fp64 and rounded once; rows [Q, Q + D) = Wq.
@@ -193,21 +210,35 @@ static int prep_copy(cudaStream_t s, const float* src, int K, int N, const float
   return MT3_OK;
 }
 
-static int prep_tc_weight(Model* m, cudaStream_t s, const float* w, int K, int N, float*& cursor, TcW* out) {
+// K-major copy (hi/lo in TF32X3) of w [K, N] for the wgmma path: carved from c and, unless c only measures, filled
+static int prep_tc_weight(Model* m, cudaStream_t s, const float* w, int K, int N, Carve& c, TcW* out) {
   out->K = K; out->N = N;
-  out->hi = cursor; cursor += (int64_t)K * N;
-  if (m->split3) { out->lo = cursor; cursor += (int64_t)K * N; }
+  out->hi = c.take((int64_t)K * N);
+  out->lo = c.take(m->split3 ? (int64_t)K * N : 0);
+  if (!c.base) return MT3_OK;
   transpose_split_kernel<<<dim3(cdiv(N, 32), cdiv(K, 32)), dim3(32, 8), 0, s>>>(w, K, N, out->hi, out->lo);
   MT3_LAUNCH_CHECK();
   return make_operand(&out->op, out->hi, out->lo, N, K, K);
 }
 
-static int64_t tc_weight_floats(const mt3_model_config& c) {
-  const int64_t D = c.emb_dim, Q = (int64_t)c.num_heads * c.head_dim, F = c.mlp_dim;
-  int64_t n = (int64_t)c.input_depth * D;
-  n += (int64_t)c.num_encoder_layers * (D * 3 * Q + Q * D + D * 2 * F + F * D);
-  n += (int64_t)c.num_decoder_layers * (D * 2 * Q);
-  return n * (c.gemm_mode == MT3_GEMM_TF32X3 ? 2 : 1);
+// A weight slab: fill(Carve&) runs once to measure it (launching nothing), then on the allocation, whose launches are
+// waited for.  *out is set on success only.
+template <class Fill>
+static int make_slab(float** out, const char* what, cudaStream_t s, Fill fill) {
+  Carve c{nullptr, sizeof(float)};
+  MT3_TRY(fill(c));
+  char* slab = nullptr;
+  cudaError_t e = cudaMalloc((void**)&slab, (size_t)c.used);
+  if (e != cudaSuccess) return fail(MT3_ERR_CUDA, "%s: cudaMalloc -> %s", what, cudaGetErrorString(e));
+  c = Carve{slab, sizeof(float)};
+  int rc = fill(c);
+  if (rc == MT3_OK && (e = cudaStreamSynchronize(s)) != cudaSuccess) rc = fail(MT3_ERR_CUDA, "%s -> %s", what, cudaGetErrorString(e));
+  if (rc != MT3_OK) {
+    cudaFree(slab);
+    return rc;
+  }
+  *out = (float*)slab;
+  return MT3_OK;
 }
 
 // The epilogue of an encoder-side GEMM C[M, N] = A[M, K] . W[K, N], in the wgmma kernel's terms (enc_gemm() maps it onto
@@ -239,6 +270,12 @@ static int make_act(const Model* m, float* hi, float* lo, int64_t rows, int cols
   a->hi = hi; a->lo = lo;
   return m->tc ? make_operand(&a->op, hi, lo, (uint64_t)rows, (uint64_t)cols, (uint64_t)cols, box_rows) : MT3_OK;
 }
+// make_act on an activation carved from c, with a lo plane when `lo`
+static int carve_act(const Model* m, Carve& c, int64_t rows, int cols, bool lo, Act* a, uint32_t box_rows = 128) {
+  float* hi = c.take(rows * cols);
+  float* l = c.take(lo ? rows * cols : 0);
+  return c.base ? make_act(m, hi, l, rows, cols, a, box_rows) : MT3_OK;
+}
 
 // x [M, K], owned by the caller, as the A operand of an encoder-side GEMM; in TF32X3 mode it is split into `pair` first.
 static int enc_input(const Model* m, const float* x, int64_t M, int K, const Act& pair, Act* out, cudaStream_t s) {
@@ -257,54 +294,68 @@ static bool tc_attention(const Model* m, int Tq, int Tk, bool causal) {
   return m->tc && m->tc_attn_ok && attention_tc_supported(Tq, Tk, causal);
 }
 
-// The layer steps of a full sequence, shared by the encoder (network.py:44-85) and the teacher-forced decoder pass
-// (:88-155): M rows of the residual stream h.  RMSNorm statistic of h, applied as the next GEMM's row scale
-static int seq_rstd(const Model* m, const Act& h, int M, float* rstd, cudaStream_t s) {
-  return launch_row_rstd(h.hi, h.lo, m->D, M, m->D, 1e-6f, rstd, s);
-}
-// QKV projection into qkv [M, 3Q].  vt: the wgmma self-attention's operands, which need qkv as a tf32 hi/lo pair (TF32X3)
-// and the V third also transposed per head into vt [B*H*64, T] (T rows per sequence): the K-major operand of P.V
-static int seq_qkv(const Model* m, const Act& h, int M, const float* rstd, const float* w, const TcW& tw, const Act& qkv, const Act* vt,
-                   int T, cudaStream_t s) {
-  const int Q = m->Q;
-  TcGemmArgs a = gemm_epi(M, 3 * Q, m->D, qkv.hi, vt ? qkv.lo : nullptr, 3 * Q);
-  a.row_scale = rstd;
-  if (vt) {
-    a.VT_hi = vt->hi; a.VT_lo = vt->lo; a.vt_col0 = 2 * Q; a.vt_T = T; a.vt_H = m->H;
-  }
-  return enc_gemm(m, h, w, tw, a, s);
-}
-// Self-attention of B sequences of T rows from qkv into ao: on the wgmma kernel when vt (seq_qkv) is given, else exact fp32.
-// key_valid [B, n_valid]: causal with per-key validity (make_decoder_mask); null: every key visible.  split_p: P . V in
-// 3xTF32 too (TF32X3; see attention_tc_kernel's PSPLIT).
-static int seq_self_attention(const Model* m, const Act& qkv, const Act* vt, int B, int T, const int* key_valid, int n_valid, bool split_p,
-                              const Act& ao, float* scratch, cudaStream_t s) {
-  const int Q = m->Q;
-  if (vt)
-    return launch_attention_tc(qkv.op, 0, T, qkv.op, Q, T, vt->op, B, m->H, ao.hi, ao.lo, m->split3, split_p, key_valid != nullptr,
-                               key_valid, n_valid, s, scratch);
-  return launch_attention_fp32(qkv.hi, 3 * Q, 0, qkv.hi, 3 * Q, Q, 2 * Q, T, T, m->H, B, ao.hi, ao.lo, Q, key_valid, n_valid, s);
-}
-// h += A . W: the attention out-projections (A = attention output) and the MLP out-projection (A = g)
-static int seq_residual(const Model* m, const Act& h, int M, const Act& A, int K, const float* w, const TcW& tw, cudaStream_t s) {
-  const int D = m->D;
-  TcGemmArgs a = gemm_epi(M, D, K, h.hi, h.lo, D);
-  a.epi = EPI_RESIDUAL; a.R_hi = h.hi; a.R_lo = h.lo; a.ldr = D;
-  return enc_gemm(m, A, w, tw, a, s);
-}
-// gated-GELU MLP-in into g [M, F]
-static int seq_mlp_in(const Model* m, const Act& h, int M, const float* rstd, const float* w, const TcW& tw, const Act& g, cudaStream_t s) {
-  const int F = m->F;
-  TcGemmArgs a = gemm_epi(M, 2 * F, m->D, g.hi, g.lo, F);
-  a.row_scale = rstd; a.epi = EPI_GATED_GELU;
-  return enc_gemm(m, h, w, tw, a, s);
+// The activations of B sequences of T rows; other_scratch: floats of attention scratch another attention of the same pass
+// shares with the self-attention's
+static int carve_seq(const Model* m, Carve& c, int B, int T, bool causal, int64_t other_scratch, SeqActs* a) {
+  const int64_t M = (int64_t)B * T;
+  const bool s3 = m->split3;
+  a->B = B; a->T = T;
+  a->tc_attn = tc_attention(m, T, T, causal);
+  MT3_TRY(carve_act(m, c, M, m->D, s3, &a->h));
+  a->rstd = c.take(M);
+  MT3_TRY(carve_act(m, c, M, 3 * m->Q, s3 && a->tc_attn, &a->qkv));
+  if (a->tc_attn) MT3_TRY(carve_act(m, c, (int64_t)B * m->H * 64, T, s3, &a->vt, 64));
+  MT3_TRY(carve_act(m, c, M, m->Q, s3, &a->ao));
+  MT3_TRY(carve_act(m, c, M, m->F, s3, &a->g));
+  a->scratch = c.take(std::max(a->tc_attn ? attention_tc_scratch_floats(B, T, T, m->H, causal) : 0, other_scratch));
+  return MT3_OK;
 }
 
-// the encoder's V^T target where its attention runs on the wgmma kernel, else null
-static const Act* enc_vt(const Model* m) { return tc_attention(m, m->T, m->T, false) ? &m->a_vt : nullptr; }
+// The layer steps of a full sequence, shared by the encoder (network.py:44-85) and the teacher-forced decoder pass
+// (:88-155), on the B * T rows of a.h.  RMSNorm statistic of h, applied as the next GEMM's row scale
+static int seq_rstd(const Model* m, const SeqActs& a, cudaStream_t s) {
+  return launch_row_rstd(a.h.hi, a.h.lo, m->D, a.B * a.T, m->D, 1e-6f, a.rstd, s);
+}
+// QKV projection into qkv [B*T, 3Q].  The wgmma self-attention needs qkv as a tf32 hi/lo pair (TF32X3) and the V third
+// also transposed per head into vt: the K-major operand of P.V
+static int seq_qkv(const Model* m, const SeqActs& a, const float* w, const TcW& tw, cudaStream_t s) {
+  const int Q = m->Q;
+  TcGemmArgs e = gemm_epi(a.B * a.T, 3 * Q, m->D, a.qkv.hi, a.qkv.lo, 3 * Q);
+  e.row_scale = a.rstd;
+  if (a.tc_attn) {
+    e.VT_hi = a.vt.hi; e.VT_lo = a.vt.lo; e.vt_col0 = 2 * Q; e.vt_T = a.T; e.vt_H = m->H;
+  }
+  return enc_gemm(m, a.h, w, tw, e, s);
+}
+// Self-attention from qkv into ao: on the wgmma kernel where tc_attn, else exact fp32.  key_valid [B, n_valid]: causal
+// with per-key validity (make_decoder_mask); null: every key visible.  split_p: P . V in 3xTF32 too (TF32X3; see
+// attention_tc_kernel's PSPLIT).
+static int seq_self_attention(const Model* m, const SeqActs& a, const int* key_valid, int n_valid, bool split_p, cudaStream_t s) {
+  const int Q = m->Q;
+  if (a.tc_attn)
+    return launch_attention_tc(a.qkv.op, 0, a.T, a.qkv.op, Q, a.T, a.vt.op, a.B, m->H, a.ao.hi, a.ao.lo, m->split3, split_p,
+                               key_valid != nullptr, key_valid, n_valid, s, a.scratch);
+  return launch_attention_fp32(a.qkv.hi, 3 * Q, 0, a.qkv.hi, 3 * Q, Q, 2 * Q, a.T, a.T, m->H, a.B, a.ao.hi, a.ao.lo, Q, key_valid, n_valid,
+                               s);
+}
+// h += A . W: the attention out-projections (A = attention output) and the MLP out-projection (A = g)
+static int seq_residual(const Model* m, const SeqActs& a, const Act& A, int K, const float* w, const TcW& tw, cudaStream_t s) {
+  const int D = m->D;
+  TcGemmArgs e = gemm_epi(a.B * a.T, D, K, a.h.hi, a.h.lo, D);
+  e.epi = EPI_RESIDUAL; e.R_hi = a.h.hi; e.R_lo = a.h.lo; e.ldr = D;
+  return enc_gemm(m, A, w, tw, e, s);
+}
+// gated-GELU MLP-in into g [B*T, F]
+static int seq_mlp_in(const Model* m, const SeqActs& a, const float* w, const TcW& tw, cudaStream_t s) {
+  const int F = m->F;
+  TcGemmArgs e = gemm_epi(a.B * a.T, 2 * F, m->D, a.g.hi, a.g.lo, F);
+  e.row_scale = a.rstd; e.epi = EPI_GATED_GELU;
+  return enc_gemm(m, a.h, w, tw, e, s);
+}
 
 // Encoder (network.py:158-193): input projection + PE, the layers, and the closing RMSNorm into `encoded`.
 static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s) {
+  const SeqActs& a = m->ea;
   const int M = m->B * m->T, D = m->D, depth = m->cfg.input_depth;
   // the exact-fp32 attention kernel's limit, in every mode
   MT3_REQUIRE(attention_fp32_smem(m->T) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED, "encode: input_length %d too long for the attention kernel",
@@ -312,23 +363,25 @@ static int encode_impl(Model* m, const float* x, float* encoded, cudaStream_t s)
   Act ax;
   MT3_TRY(enc_input(m, x, M, depth, m->a_x, &ax, s));
   {
-    TcGemmArgs a = gemm_epi(M, D, depth, m->a_h.hi, m->a_h.lo, D);
-    a.epi = EPI_ADD_PE; a.pe = m->pe; a.pe_T = m->T; a.pe_ld = D;
-    MT3_TRY(enc_gemm(m, ax, m->w_in, m->t_w_in, a, s));
+    TcGemmArgs e = gemm_epi(M, D, depth, a.h.hi, a.h.lo, D);
+    e.epi = EPI_ADD_PE; e.pe = m->pe; e.pe_T = m->T; e.pe_ld = D;
+    MT3_TRY(enc_gemm(m, ax, m->w_in, m->t_w_in, e, s));
   }
-  const Act* vt = enc_vt(m);
   for (int l = 0; l < m->Le; ++l) {
     const EncLayer& w = m->enc[l];
-    MT3_TRY(seq_rstd(m, m->a_h, M, m->rstd, s));
-    MT3_TRY(seq_qkv(m, m->a_h, M, m->rstd, w.wqkv, w.t_wqkv, m->a_qkv, vt, m->T, s));
-    MT3_TRY(seq_self_attention(m, m->a_qkv, vt, m->B, m->T, nullptr, 0, false, m->a_ao, m->att_scratch, s));
-    MT3_TRY(seq_residual(m, m->a_h, M, m->a_ao, m->Q, w.wo, w.t_wo, s));
-    MT3_TRY(seq_rstd(m, m->a_h, M, m->rstd, s));
-    MT3_TRY(seq_mlp_in(m, m->a_h, M, m->rstd, w.wi, w.t_wi, m->a_g, s));
-    MT3_TRY(seq_residual(m, m->a_h, M, m->a_g, m->F, w.wo2, w.t_wo2, s));
+    MT3_TRY(seq_rstd(m, a, s));
+    MT3_TRY(seq_qkv(m, a, w.wqkv, w.t_wqkv, s));
+    MT3_TRY(seq_self_attention(m, a, nullptr, 0, false, s));
+    MT3_TRY(seq_residual(m, a, a.ao, m->Q, w.wo, w.t_wo, s));
+    MT3_TRY(seq_rstd(m, a, s));
+    MT3_TRY(seq_mlp_in(m, a, w.wi, w.t_wi, s));
+    MT3_TRY(seq_residual(m, a, a.g, m->F, w.wo2, w.t_wo2, s));
   }
-  return launch_rmsnorm(m->a_h.hi, m->a_h.lo, D, M, D, 1e-6f, m->enc_norm_g, encoded, D, s);
+  return launch_rmsnorm(a.h.hi, a.h.lo, D, M, D, 1e-6f, m->enc_norm_g, encoded, D, s);
 }
+
+// Output tiles of the widest decode GEMM (QKV, MLP-in or logits): the length of the decode GEMMs' tile counters
+static int dec_tiles(const Model* m) { return cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN); }
 
 // The hoisted cross-attention K/V of every decoder layer, head-major, and the reset of the decode state.
 static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
@@ -341,7 +394,7 @@ static int cross_kv_impl(Model* m, const float* encoded, cudaStream_t s) {
     MT3_TRY(enc_gemm(m, ae, m->dec[l].wkv_c, m->dec[l].t_wkv_c, a, s));
   }
   MT3_CUDA_CHECK(cudaMemsetAsync(m->state, 0, 4 * sizeof(int), s));
-  MT3_CUDA_CHECK(cudaMemsetAsync(m->dcounters, 0, (size_t)m->dcounters_n * sizeof(int), s));
+  MT3_CUDA_CHECK(cudaMemsetAsync(m->dcounters, 0, (size_t)dec_tiles(m) * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->finished, 0, (size_t)m->B * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->tok_cur, 0, (size_t)m->B * sizeof(int), s));
   m->have_cross = true;
@@ -518,10 +571,10 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
   float* tok_scores = scored ? m->tok_scores : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->beam_f,
-                              m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, m->pe_rows, m->D, y_next, s));
+                              m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, kPeRows, m->D, y_next, s));
   } else if (greedy) {
     MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
-                               tok_scores, m->L, loop_step ? m->plen : nullptr, tok_user, m->state, 1, 0, m->emb, m->pe, m->pe_rows, m->D,
+                               tok_scores, m->L, loop_step ? m->plen : nullptr, tok_user, m->state, 1, 0, m->emb, m->pe, kPeRows, m->D,
                                y_next, m->B, s));
   } else {
     MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
@@ -605,77 +658,68 @@ constexpr int kTfLogitRows = 8192;   // logits rows per chunk of the logits GEMM
 
 static int tf_pad(int L) { return cdiv(L, kAtQ) * kAtQ; }
 
-struct TfLayout {
-  int64_t y, y_lo, rstd, qkv, qkv_lo, vt, vt_lo, ao, ao_lo, qc, qc_lo, enc, enc_lo, ckv, ckv_lo, cvt, cvt_lo, g, g_lo, scratch, logits, total;
+// The pass's workspace: the full-sequence activations of B sequences of Lp causal rows, and what the cross-attention and
+// the logits add: the queries qc, `encoded` as a tf32 hi/lo pair (TF32X3), one layer's cross K | V [B*T, 2Q] (V also as
+// V^T in cvt where the cross-attention runs on the wgmma kernel, tcc) and one chunk of logits rows.
+struct TfActs {
+  SeqActs seq;
+  bool tcc = false;
+  Act qc, enc_pair, ckv, cvt;
+  float* logits = nullptr;
 };
-static TfLayout tf_layout(const Model* m, int B, int T, int L) {
-  TfLayout w;
-  int64_t off = 0;
-  auto take = [&](int64_t bytes) { int64_t r = off; off += align_up(bytes, 256); return r; };
+static int carve_tf(const Model* m, Carve& c, int B, int T, int L, TfActs* w) {
   const int Lp = tf_pad(L);
-  const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T, D = m->D, Q = m->Q, F = m->F, V = m->V;
-  const bool s3 = m->split3, tcs = tc_attention(m, Lp, Lp, true), tcc = tc_attention(m, Lp, T, false);
-  w.y = take(M * D * 4);                          // residual stream (hi/lo in TF32X3)
-  w.y_lo = take(s3 ? M * D * 4 : 0);
-  w.rstd = take(M * 4);
-  w.qkv = take(M * 3 * Q * 4);
-  w.qkv_lo = take(s3 && tcs ? M * 3 * Q * 4 : 0);
-  w.vt = take(tcs ? M * Q * 4 : 0);               // per-head V^T [B*H*64, Lp] of the wgmma self-attention
-  w.vt_lo = take(s3 && tcs ? M * Q * 4 : 0);
-  w.ao = take(M * Q * 4);                         // attention output (self, then cross)
-  w.ao_lo = take(s3 ? M * Q * 4 : 0);
-  w.qc = take(M * Q * 4);                         // cross-attention queries
-  w.qc_lo = take(s3 && tcc ? M * Q * 4 : 0);
-  w.enc = take(s3 ? Me * D * 4 : 0);              // tf32 hi/lo split of `encoded` (TF32X3)
-  w.enc_lo = take(s3 ? Me * D * 4 : 0);
-  w.ckv = take(Me * 2 * Q * 4);                   // one layer's cross K | V [B*T, 2Q] (V as V^T in cvt on the wgmma path)
-  w.ckv_lo = take(s3 && tcc ? Me * 2 * Q * 4 : 0);
-  w.cvt = take(tcc ? Me * Q * 4 : 0);
-  w.cvt_lo = take(s3 && tcc ? Me * Q * 4 : 0);
-  w.g = take(M * F * 4);
-  w.g_lo = take(s3 ? M * F * 4 : 0);
-  w.scratch = take(std::max(tcs ? attention_tc_scratch_floats(B, Lp, Lp, m->H, true) : 0,
-                            tcc ? attention_tc_scratch_floats(B, Lp, T, m->H, false) : 0) * 4);
-  w.logits = take(std::min(M, (int64_t)kTfLogitRows) * V * 4);
-  w.total = off;
-  return w;
+  const int64_t M = (int64_t)B * Lp, Me = (int64_t)B * T;
+  const bool s3 = m->split3;
+  w->tcc = tc_attention(m, Lp, T, false);
+  MT3_TRY(carve_seq(m, c, B, Lp, true, w->tcc ? attention_tc_scratch_floats(B, Lp, T, m->H, false) : 0, &w->seq));
+  MT3_TRY(carve_act(m, c, M, m->Q, s3 && w->tcc, &w->qc));
+  if (s3) MT3_TRY(carve_act(m, c, Me, m->D, true, &w->enc_pair));
+  MT3_TRY(carve_act(m, c, Me, 2 * m->Q, s3 && w->tcc, &w->ckv));
+  if (w->tcc) MT3_TRY(carve_act(m, c, (int64_t)B * m->H * 64, T, s3, &w->cvt, 64));
+  w->logits = c.take(std::min(M, (int64_t)kTfLogitRows) * m->V);
+  return MT3_OK;
 }
 
-static int64_t tf_weight_floats(const Model* m) {
-  const int64_t D = m->D, Q = m->Q, F = m->F, V = m->V;
-  const int64_t per_layer = D * 3 * Q + Q * D + D * Q + Q * D + D * 2 * F + F * D;
-  return (m->Ld * per_layer + D * V) * (m->split3 ? 2 : 1);
+static int64_t tf_workspace_bytes(const Model* m, int B, int T, int L) {
+  Carve c;
+  TfActs w;
+  carve_tf(m, c, B, T, L, &w);
+  return c.used;
+}
+
+// The caller's workspace for the pass over B x L targets and T inputs: non-null, 256-byte aligned and large enough
+static int check_tf_workspace(const Model* m, const char* name, const void* ws, int64_t bytes, int B, int T, int L) {
+  MT3_REQUIRE(ws && ((uintptr_t)ws & 255) == 0, MT3_ERR_WORKSPACE, "%s: the teacher-forced workspace must be non-null and 256-byte aligned",
+              name);
+  const int64_t need = tf_workspace_bytes(m, B, T, L);
+  MT3_REQUIRE(bytes >= need, MT3_ERR_WORKSPACE, "%s: workspace has %lld bytes, %lld needed", name, (long long)bytes, (long long)need);
+  return MT3_OK;
+}
+
+// Whether the pass takes L targets over T inputs: the exact-fp32 attention kernel's limits wherever it runs
+static bool tf_supported(const Model* m, int T, int L) {
+  const int Lp = tf_pad(L);
+  return (tc_attention(m, Lp, Lp, true) || attention_fp32_smem(Lp) <= kAttFp32MaxSmem) &&
+         (tc_attention(m, Lp, T, false) || attention_fp32_smem(T) <= kAttFp32MaxSmem);
 }
 
 // K-major (hi/lo in TF32X3) copies of the decoder weights the pass multiplies on the wgmma path: made on its first call,
 // so that a model that only transcribes keeps its footprint (TF32X3 ~183 MB, TF32 ~92 MB at the mt3 shapes).
 static int ensure_tf_weights(Model* m, cudaStream_t s) {
   if (!m->tc || m->slab_tf) return MT3_OK;
-  float* slab = nullptr;
-  MT3_CUDA_CHECK(cudaMalloc((void**)&slab, (size_t)tf_weight_floats(m) * sizeof(float)));
-  float* cur = slab;
   const int D = m->D, Q = m->Q, F = m->F;
-  int rc = MT3_OK;
-  for (int l = 0; l < m->Ld && rc == MT3_OK; ++l) {
-    DecLayer& L = m->dec[l];
-    rc = prep_tc_weight(m, s, L.wqkv, D, 3 * Q, cur, &L.t_wqkv);
-    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo, Q, D, cur, &L.t_wo);
-    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wq_c, D, Q, cur, &L.t_wq_c);
-    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo_c, Q, D, cur, &L.t_wo_c);
-    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wi, D, 2 * F, cur, &L.t_wi);
-    if (rc == MT3_OK) rc = prep_tc_weight(m, s, L.wo2, F, D, cur, &L.t_wo2);
-  }
-  if (rc == MT3_OK) rc = prep_tc_weight(m, s, m->w_logits, D, m->V, cur, &m->t_w_logits);
-  if (rc == MT3_OK) {
-    const cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "teacher-forced weight prep -> %s", cudaGetErrorString(e));
-  }
-  if (rc != MT3_OK) {
-    cudaFree(slab);
-    return rc;
-  }
-  m->slab_tf = slab;
-  return MT3_OK;
+  return make_slab(&m->slab_tf, "teacher-forced weight prep", s, [&](Carve& c) -> int {
+    for (DecLayer& L : m->dec) {
+      MT3_TRY(prep_tc_weight(m, s, L.wqkv, D, 3 * Q, c, &L.t_wqkv));
+      MT3_TRY(prep_tc_weight(m, s, L.wo, Q, D, c, &L.t_wo));
+      MT3_TRY(prep_tc_weight(m, s, L.wq_c, D, Q, c, &L.t_wq_c));
+      MT3_TRY(prep_tc_weight(m, s, L.wo_c, Q, D, c, &L.t_wo_c));
+      MT3_TRY(prep_tc_weight(m, s, L.wi, D, 2 * F, c, &L.t_wi));
+      MT3_TRY(prep_tc_weight(m, s, L.wo2, F, D, c, &L.t_wo2));
+    }
+    return prep_tc_weight(m, s, m->w_logits, D, m->V, c, &m->t_w_logits);
+  });
 }
 
 // Positions t < n of every sequence of the pass's self-attention K/V -> the decode cache: head-major rows [b][K|V][h][cap] at
@@ -709,68 +753,60 @@ __global__ void prefill_kv_kernel(const float* __restrict__ qkv_hi, const float*
 // are not computed.
 static int teacher_forced_impl(Model* m, const float* encoded, int B, int T, const int* tok_in, const int* tgt, const int* wts, int L,
                                float* logits, float* scores, char* ws, cudaStream_t s, char* kv_cache = nullptr) {
-  const int Lp = tf_pad(L), D = m->D, Q = m->Q, F = m->F, V = m->V, H = m->H;
+  TfActs w;
+  Carve c{ws};
+  MT3_TRY(carve_tf(m, c, B, T, L, &w));
+  const SeqActs& y = w.seq;
+  const int Lp = y.T, D = m->D, Q = m->Q, F = m->F, V = m->V, H = m->H;
   const int M = B * Lp, Me = B * T;
-  const bool s3 = m->split3, tcs = tc_attention(m, Lp, Lp, true), tcc = tc_attention(m, Lp, T, false);
-  const TfLayout w = tf_layout(m, B, T, L);
-  auto P = [&](int64_t off, bool on = true) { return on ? (float*)(ws + off) : nullptr; };
-  Act y, qkv, vt, ao, qc, enc_pair, enc, ckv, cvt, g;
-  MT3_TRY(make_act(m, P(w.y), P(w.y_lo, s3), M, D, &y));
-  MT3_TRY(make_act(m, P(w.ao), P(w.ao_lo, s3), M, Q, &ao));
-  MT3_TRY(make_act(m, P(w.g), P(w.g_lo, s3), M, F, &g));
-  MT3_TRY(make_act(m, P(w.qkv), P(w.qkv_lo, s3 && tcs), M, 3 * Q, &qkv));
-  MT3_TRY(make_act(m, P(w.qc), P(w.qc_lo, s3 && tcc), M, Q, &qc));
-  MT3_TRY(make_act(m, P(w.ckv), P(w.ckv_lo, s3 && tcc), Me, 2 * Q, &ckv));
-  if (tcs) MT3_TRY(make_act(m, P(w.vt), P(w.vt_lo, s3), (int64_t)B * H * 64, Lp, &vt, 64));
-  if (tcc) MT3_TRY(make_act(m, P(w.cvt), P(w.cvt_lo, s3), (int64_t)B * H * 64, T, &cvt, 64));
-  if (s3) MT3_TRY(make_act(m, P(w.enc), P(w.enc_lo), Me, D, &enc_pair));
-  MT3_TRY(enc_input(m, encoded, Me, D, enc_pair, &enc, s));
-  float* rstd = P(w.rstd);
-  float* scratch = P(w.scratch, w.logits > w.scratch);
+  Act enc;
+  MT3_TRY(enc_input(m, encoded, Me, D, w.enc_pair, &enc, s));
 
-  MT3_TRY(launch_embed_seq(tok_in, B, L, Lp, m->emb, D, V, m->pe, y.hi, y.lo, s));
+  MT3_TRY(launch_embed_seq(tok_in, B, L, Lp, m->emb, D, V, m->pe, y.h.hi, y.h.lo, s));
   for (int l = 0; l < m->Ld; ++l) {
     const DecLayer& dl = m->dec[l];
     // self-attention: RMSNorm folded into the QKV projection's row scale; mask make_decoder_mask(targets)
-    MT3_TRY(seq_rstd(m, y, M, rstd, s));
-    MT3_TRY(seq_qkv(m, y, M, rstd, dl.wqkv, dl.t_wqkv, qkv, tcs ? &vt : nullptr, Lp, s));
+    MT3_TRY(seq_rstd(m, y, s));
+    MT3_TRY(seq_qkv(m, y, dl.wqkv, dl.t_wqkv, s));
     if (kv_cache) {
-      prefill_kv_kernel<<<dim3(L, B), 128, 0, s>>>(qkv.hi, qkv.lo, tcs ? vt.hi : nullptr, tcs ? vt.lo : nullptr, Lp, H, m->kv_fmt,
-                                                   kv_layer(m, kv_cache, l, m->L), m->L);
+      prefill_kv_kernel<<<dim3(L, B), 128, 0, s>>>(y.qkv.hi, y.qkv.lo, y.vt.hi, y.vt.lo, Lp, H, m->kv_fmt, kv_layer(m, kv_cache, l, m->L),
+                                                   m->L);
       MT3_LAUNCH_CHECK();
       if (l == m->Ld - 1) return MT3_OK;
     }
-    MT3_TRY(seq_self_attention(m, qkv, tcs ? &vt : nullptr, B, Lp, tgt, L, true, ao, scratch, s));
-    MT3_TRY(seq_residual(m, y, M, ao, Q, dl.wo, dl.t_wo, s));
+    MT3_TRY(seq_self_attention(m, y, tgt, L, true, s));
+    MT3_TRY(seq_residual(m, y, y.ao, Q, dl.wo, dl.t_wo, s));
     // cross-attention over all T encoder positions; K/V projected from `encoded` for this layer
-    MT3_TRY(seq_rstd(m, y, M, rstd, s));
+    MT3_TRY(seq_rstd(m, y, s));
     {
-      TcGemmArgs a = gemm_epi(M, Q, D, qc.hi, qc.lo, Q);
-      a.row_scale = rstd;
-      MT3_TRY(enc_gemm(m, y, dl.wq_c, dl.t_wq_c, a, s));
+      TcGemmArgs a = gemm_epi(M, Q, D, w.qc.hi, w.qc.lo, Q);
+      a.row_scale = y.rstd;
+      MT3_TRY(enc_gemm(m, y.h, dl.wq_c, dl.t_wq_c, a, s));
     }
     {
-      TcGemmArgs a = gemm_epi(Me, 2 * Q, D, ckv.hi, ckv.lo, 2 * Q);
-      if (tcc) { a.VT_hi = cvt.hi; a.VT_lo = cvt.lo; a.vt_col0 = Q; a.vt_T = T; a.vt_H = H; }
+      TcGemmArgs a = gemm_epi(Me, 2 * Q, D, w.ckv.hi, w.ckv.lo, 2 * Q);
+      if (w.tcc) { a.VT_hi = w.cvt.hi; a.VT_lo = w.cvt.lo; a.vt_col0 = Q; a.vt_T = T; a.vt_H = H; }
       MT3_TRY(enc_gemm(m, enc, dl.wkv_c, dl.t_wkv_c, a, s));
     }
-    if (tcc) MT3_TRY(launch_attention_tc(qc.op, 0, Lp, ckv.op, 0, T, cvt.op, B, H, ao.hi, ao.lo, s3, true, false, nullptr, 0, s, scratch));
-    else MT3_TRY(launch_attention_fp32(qc.hi, Q, 0, ckv.hi, 2 * Q, 0, Q, Lp, T, H, B, ao.hi, ao.lo, Q, nullptr, 0, s));
-    MT3_TRY(seq_residual(m, y, M, ao, Q, dl.wo_c, dl.t_wo_c, s));
+    if (w.tcc)
+      MT3_TRY(launch_attention_tc(w.qc.op, 0, Lp, w.ckv.op, 0, T, w.cvt.op, B, H, y.ao.hi, y.ao.lo, m->split3, true, false, nullptr, 0, s,
+                                  y.scratch));
+    else MT3_TRY(launch_attention_fp32(w.qc.hi, Q, 0, w.ckv.hi, 2 * Q, 0, Q, Lp, T, H, B, y.ao.hi, y.ao.lo, Q, nullptr, 0, s));
+    MT3_TRY(seq_residual(m, y, y.ao, Q, dl.wo_c, dl.t_wo_c, s));
     // gated-GELU MLP
-    MT3_TRY(seq_rstd(m, y, M, rstd, s));
-    MT3_TRY(seq_mlp_in(m, y, M, rstd, dl.wi, dl.t_wi, g, s));
-    MT3_TRY(seq_residual(m, y, M, g, F, dl.wo2, dl.t_wo2, s));
+    MT3_TRY(seq_rstd(m, y, s));
+    MT3_TRY(seq_mlp_in(m, y, dl.wi, dl.t_wi, s));
+    MT3_TRY(seq_residual(m, y, y.g, F, dl.wo2, dl.t_wo2, s));
   }
   // decoder_norm (folded into w_logits) + logits_dense, then the scores, in chunks of rows
-  MT3_TRY(seq_rstd(m, y, M, rstd, s));
-  float* chunk = P(w.logits);
+  MT3_TRY(seq_rstd(m, y, s));
+  float* chunk = w.logits;
   for (int64_t r0 = 0; r0 < M; r0 += kTfLogitRows) {
     const int n = (int)std::min((int64_t)kTfLogitRows, M - r0);
     Act ys;
-    MT3_TRY(make_act(m, y.hi + r0 * D, y.lo ? y.lo + r0 * D : nullptr, n, D, &ys));
+    MT3_TRY(make_act(m, y.h.hi + r0 * D, y.h.lo ? y.h.lo + r0 * D : nullptr, n, D, &ys));
     TcGemmArgs a = gemm_epi(n, V, D, chunk, nullptr, V);
-    a.row_scale = rstd + r0;
+    a.row_scale = y.rstd + r0;
     MT3_TRY(enc_gemm(m, ys, m->w_logits, m->t_w_logits, a, s));
     MT3_TRY(launch_token_score(chunk, V, (int)r0, n, Lp, L, tgt, wts, scores, logits, s));
   }
@@ -797,6 +833,80 @@ extern "C" int64_t mt3_model_param_offset(const mt3_model_config* cfg, const cha
   return -1;
 }
 
+// The prepared weights: each buffer carved from c (float counts, no padding) and, unless c only measures, filled from the
+// reference's tensors in `weights` (fused, scale-folded and precomposed as DESIGN.md §2 lists)
+static int prep_weights(Model* m, const float* weights, Carve& c, cudaStream_t s) {
+  const mt3_model_config* cfg = &m->cfg;
+  const int D = m->D, Q = m->Q, F = m->F, V = m->V;
+  const auto t = param_table(*cfg);
+  auto W = [&](const std::string& n) -> const float* {
+    for (const auto& en : t) if (en.name == n) return weights + en.offset;
+    return nullptr;
+  };
+  int rc = MT3_OK;
+#define PREP(...) do { if (rc == MT3_OK && c.base) rc = prep_copy(s, __VA_ARGS__); } while (0)
+  m->w_in = c.take((int64_t)cfg->input_depth * D);
+  PREP(W("encoder/continuous_inputs_projection/kernel"), cfg->input_depth, D, nullptr, m->w_in, D, 0, 1);
+  m->enc.resize(m->Le);
+  for (int i = 0; i < m->Le; ++i) {
+    const std::string pre = "encoder/layers_" + std::to_string(i) + "/";
+    EncLayer& L = m->enc[i];
+    const float* g1 = W(pre + "pre_attention_layer_norm/scale");
+    const float* g2 = W(pre + "pre_mlp_layer_norm/scale");
+    L.wqkv = c.take((int64_t)D * 3 * Q);
+    PREP(W(pre + "attention/query/kernel"), D, Q, g1, L.wqkv, 3 * Q, 0, 1);
+    PREP(W(pre + "attention/key/kernel"), D, Q, g1, L.wqkv, 3 * Q, Q, 1);
+    PREP(W(pre + "attention/value/kernel"), D, Q, g1, L.wqkv, 3 * Q, 2 * Q, 1);
+    L.wo = c.take((int64_t)Q * D);
+    PREP(W(pre + "attention/out/kernel"), Q, D, nullptr, L.wo, D, 0, 1);
+    L.wi = c.take((int64_t)D * 2 * F);
+    PREP(W(pre + "mlp/wi_0/kernel"), D, F, g2, L.wi, 2 * F, 0, 2);
+    PREP(W(pre + "mlp/wi_1/kernel"), D, F, g2, L.wi, 2 * F, 1, 2);
+    L.wo2 = c.take((int64_t)F * D);
+    PREP(W(pre + "mlp/wo/kernel"), F, D, nullptr, L.wo2, D, 0, 1);
+  }
+  m->enc_norm_g = c.take(D);
+  PREP(W("encoder/encoder_norm/scale"), 1, D, nullptr, m->enc_norm_g, D, 0, 1);
+  m->emb = c.take((int64_t)V * D);
+  PREP(W("decoder/token_embedder/embedding"), V, D, nullptr, m->emb, D, 0, 1);
+  m->dec.resize(m->Ld);
+  for (int i = 0; i < m->Ld; ++i) {
+    const std::string pre = "decoder/layers_" + std::to_string(i) + "/";
+    DecLayer& L = m->dec[i];
+    const float* g1 = W(pre + "pre_self_attention_layer_norm/scale");
+    const float* g2 = W(pre + "pre_cross_attention_layer_norm/scale");
+    const float* g3 = W(pre + "pre_mlp_layer_norm/scale");
+    L.wqkv = c.take((int64_t)D * 3 * Q);
+    PREP(W(pre + "self_attention/query/kernel"), D, Q, g1, L.wqkv, 3 * Q, 0, 1);
+    PREP(W(pre + "self_attention/key/kernel"), D, Q, g1, L.wqkv, 3 * Q, Q, 1);
+    PREP(W(pre + "self_attention/value/kernel"), D, Q, g1, L.wqkv, 3 * Q, 2 * Q, 1);
+    L.wo = c.take((int64_t)Q * D);
+    PREP(W(pre + "self_attention/out/kernel"), Q, D, nullptr, L.wo, D, 0, 1);
+    L.wq_c = c.take((int64_t)D * Q);
+    PREP(W(pre + "encoder_decoder_attention/query/kernel"), D, Q, g2, L.wq_c, Q, 0, 1);
+    L.wc1 = c.take((int64_t)(Q + D) * Q);
+    if (rc == MT3_OK && c.base) {
+      compose_out_q_kernel<<<dim3(cdiv(Q, 128), Q + D), 128, 0, s>>>(L.wo, L.wq_c, Q, D, L.wc1);
+      if (cudaGetLastError() != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: compose_out_q launch failed");
+    }
+    L.wkv_c = c.take((int64_t)D * 2 * Q);   // applied to `encoded`, which is already normed: no fold
+    PREP(W(pre + "encoder_decoder_attention/key/kernel"), D, Q, nullptr, L.wkv_c, 2 * Q, 0, 1);
+    PREP(W(pre + "encoder_decoder_attention/value/kernel"), D, Q, nullptr, L.wkv_c, 2 * Q, Q, 1);
+    L.wo_c = c.take((int64_t)Q * D);
+    PREP(W(pre + "encoder_decoder_attention/out/kernel"), Q, D, nullptr, L.wo_c, D, 0, 1);
+    L.wi = c.take((int64_t)D * 2 * F);
+    PREP(W(pre + "mlp/wi_0/kernel"), D, F, g3, L.wi, 2 * F, 0, 2);
+    PREP(W(pre + "mlp/wi_1/kernel"), D, F, g3, L.wi, 2 * F, 1, 2);
+    L.wo2 = c.take((int64_t)F * D);
+    PREP(W(pre + "mlp/wo/kernel"), F, D, nullptr, L.wo2, D, 0, 1);
+  }
+  m->w_logits = c.take((int64_t)D * V);
+  PREP(W("decoder/logits_dense/kernel"), D, V, W("decoder/decoder_norm/scale"), m->w_logits, V, 0, 1);
+#undef PREP
+  m->pe = c.take((int64_t)kPeRows * D);
+  return rc;
+}
+
 extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weights, mt3_model** out, void* stream) {
   MT3_REQUIRE(cfg && weights && out, MT3_ERR_BAD_ARG, "mt3_model_create: null argument");
   MT3_REQUIRE(cfg->head_dim == kHD, MT3_ERR_UNSUPPORTED, "mt3_model_create: head_dim %d (kernels are built for 64)", cfg->head_dim);
@@ -805,7 +915,7 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
   MT3_REQUIRE(cfg->num_heads > 0 && cfg->num_encoder_layers >= 0 && cfg->num_decoder_layers > 0 && cfg->max_batch > 0 &&
                   cfg->max_input_length > 0 && cfg->max_decode_length > 0,
               MT3_ERR_BAD_ARG, "mt3_model_create: non-positive size");
-  MT3_REQUIRE(cfg->max_decode_length <= 2048 && cfg->max_input_length <= 2048, MT3_ERR_UNSUPPORTED,
+  MT3_REQUIRE(cfg->max_decode_length <= kPeRows && cfg->max_input_length <= kPeRows, MT3_ERR_UNSUPPORTED,
               "mt3_model_create: lengths above FixedEmbed.max_length=2048 (layers.py:565)");
   MT3_REQUIRE(cfg->gemm_mode == MT3_GEMM_FP32_SIMT || cfg->gemm_mode == MT3_GEMM_TF32X3 || cfg->gemm_mode == MT3_GEMM_TF32,
               MT3_ERR_BAD_ARG, "mt3_model_create: unknown gemm_mode %d", cfg->gemm_mode);
@@ -820,91 +930,20 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
   m->D = cfg->emb_dim; m->H = cfg->num_heads; m->Q = cfg->num_heads * cfg->head_dim; m->F = cfg->mlp_dim;
   m->V = cfg->vocab_size; m->Le = cfg->num_encoder_layers; m->Ld = cfg->num_decoder_layers; m->L = cfg->max_decode_length;
   const int D = m->D, Q = m->Q, F = m->F, V = m->V;
-  cudaError_t e = cudaMalloc((void**)&m->slab, (size_t)prepared_floats(*cfg) * sizeof(float));
-  if (e != cudaSuccess) {
-    delete m;
-    return fail(MT3_ERR_CUDA, "mt3_model_create: cudaMalloc -> %s", cudaGetErrorString(e));
-  }
-  float* p = m->slab;
-  auto take = [&](int64_t n) { float* r = p; p += n; return r; };
-  auto t = param_table(*cfg);
-  auto W = [&](const std::string& n) -> const float* {
-    for (const auto& en : t) if (en.name == n) return weights + en.offset;
-    return nullptr;
-  };
-  int rc = MT3_OK;
-#define PREP(...) do { if (rc == MT3_OK) rc = prep_copy(s, __VA_ARGS__); } while (0)
-  m->w_in = take((int64_t)cfg->input_depth * D);
-  PREP(W("encoder/continuous_inputs_projection/kernel"), cfg->input_depth, D, nullptr, m->w_in, D, 0, 1);
-  m->enc.resize(m->Le);
-  for (int i = 0; i < m->Le; ++i) {
-    const std::string pre = "encoder/layers_" + std::to_string(i) + "/";
-    EncLayer& L = m->enc[i];
-    const float* g1 = W(pre + "pre_attention_layer_norm/scale");
-    const float* g2 = W(pre + "pre_mlp_layer_norm/scale");
-    L.wqkv = take((int64_t)D * 3 * Q);
-    PREP(W(pre + "attention/query/kernel"), D, Q, g1, L.wqkv, 3 * Q, 0, 1);
-    PREP(W(pre + "attention/key/kernel"), D, Q, g1, L.wqkv, 3 * Q, Q, 1);
-    PREP(W(pre + "attention/value/kernel"), D, Q, g1, L.wqkv, 3 * Q, 2 * Q, 1);
-    L.wo = take((int64_t)Q * D);
-    PREP(W(pre + "attention/out/kernel"), Q, D, nullptr, L.wo, D, 0, 1);
-    L.wi = take((int64_t)D * 2 * F);
-    PREP(W(pre + "mlp/wi_0/kernel"), D, F, g2, L.wi, 2 * F, 0, 2);
-    PREP(W(pre + "mlp/wi_1/kernel"), D, F, g2, L.wi, 2 * F, 1, 2);
-    L.wo2 = take((int64_t)F * D);
-    PREP(W(pre + "mlp/wo/kernel"), F, D, nullptr, L.wo2, D, 0, 1);
-  }
-  m->enc_norm_g = take(D);
-  PREP(W("encoder/encoder_norm/scale"), 1, D, nullptr, m->enc_norm_g, D, 0, 1);
-  m->emb = take((int64_t)V * D);
-  PREP(W("decoder/token_embedder/embedding"), V, D, nullptr, m->emb, D, 0, 1);
-  m->dec.resize(m->Ld);
-  for (int i = 0; i < m->Ld; ++i) {
-    const std::string pre = "decoder/layers_" + std::to_string(i) + "/";
-    DecLayer& L = m->dec[i];
-    const float* g1 = W(pre + "pre_self_attention_layer_norm/scale");
-    const float* g2 = W(pre + "pre_cross_attention_layer_norm/scale");
-    const float* g3 = W(pre + "pre_mlp_layer_norm/scale");
-    L.wqkv = take((int64_t)D * 3 * Q);
-    PREP(W(pre + "self_attention/query/kernel"), D, Q, g1, L.wqkv, 3 * Q, 0, 1);
-    PREP(W(pre + "self_attention/key/kernel"), D, Q, g1, L.wqkv, 3 * Q, Q, 1);
-    PREP(W(pre + "self_attention/value/kernel"), D, Q, g1, L.wqkv, 3 * Q, 2 * Q, 1);
-    L.wo = take((int64_t)Q * D);
-    PREP(W(pre + "self_attention/out/kernel"), Q, D, nullptr, L.wo, D, 0, 1);
-    L.wq_c = take((int64_t)D * Q);
-    PREP(W(pre + "encoder_decoder_attention/query/kernel"), D, Q, g2, L.wq_c, Q, 0, 1);
-    L.wc1 = take((int64_t)(Q + D) * Q);
-    if (rc == MT3_OK) {
-      compose_out_q_kernel<<<dim3(cdiv(Q, 128), Q + D), 128, 0, s>>>(L.wo, L.wq_c, Q, D, L.wc1);
-      if (cudaGetLastError() != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: compose_out_q launch failed");
-    }
-    L.wkv_c = take((int64_t)D * 2 * Q);   // applied to `encoded`, which is already normed: no fold
-    PREP(W(pre + "encoder_decoder_attention/key/kernel"), D, Q, nullptr, L.wkv_c, 2 * Q, 0, 1);
-    PREP(W(pre + "encoder_decoder_attention/value/kernel"), D, Q, nullptr, L.wkv_c, 2 * Q, Q, 1);
-    L.wo_c = take((int64_t)Q * D);
-    PREP(W(pre + "encoder_decoder_attention/out/kernel"), Q, D, nullptr, L.wo_c, D, 0, 1);
-    L.wi = take((int64_t)D * 2 * F);
-    PREP(W(pre + "mlp/wi_0/kernel"), D, F, g3, L.wi, 2 * F, 0, 2);
-    PREP(W(pre + "mlp/wi_1/kernel"), D, F, g3, L.wi, 2 * F, 1, 2);
-    L.wo2 = take((int64_t)F * D);
-    PREP(W(pre + "mlp/wo/kernel"), F, D, nullptr, L.wo2, D, 0, 1);
-  }
-  m->w_logits = take((int64_t)D * V);
-  PREP(W("decoder/logits_dense/kernel"), D, V, W("decoder/decoder_norm/scale"), m->w_logits, V, 0, 1);
-#undef PREP
-  m->pe = take((int64_t)m->pe_rows * D);
+  int rc = make_slab(&m->slab, "mt3_model_create: prepared weights", s,
+                     [&](Carve& c) { return prep_weights(m, weights, c, s); });
   if (rc == MT3_OK) {
     // layers.py:51-82 (float64 on the host, rounded to float32 like the reference's numpy code)
-    std::vector<float> pe((size_t)m->pe_rows * D, 0.f);
+    std::vector<float> pe((size_t)kPeRows * D, 0.f);
     const int half = D / 2;
     const double scale_factor = -log(10000.0 / 1.0) / (double)(half - 1);
-    for (int pos = 0; pos < m->pe_rows; ++pos)
+    for (int pos = 0; pos < kPeRows; ++pos)
       for (int i = 0; i < half; ++i) {
         const double div = 1.0 * exp((double)i * scale_factor);
         pe[(size_t)pos * D + i] = (float)sin((double)pos * div);
         pe[(size_t)pos * D + half + i] = (float)cos((double)pos * div);
       }
-    e = cudaMemcpyAsync(m->pe, pe.data(), pe.size() * sizeof(float), cudaMemcpyHostToDevice, s);
+    cudaError_t e = cudaMemcpyAsync(m->pe, pe.data(), pe.size() * sizeof(float), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: PE upload -> %s", cudaGetErrorString(e));
   }
@@ -924,28 +963,20 @@ extern "C" int mt3_model_create(const mt3_model_config* cfg, const float* weight
   m->kv_row = kv_row_bytes(m->kv_fmt);
   m->tc = cfg->gemm_mode != MT3_GEMM_FP32_SIMT;
   m->split3 = cfg->gemm_mode == MT3_GEMM_TF32X3;
-  if (rc == MT3_OK && m->tc) {
-    e = cudaMalloc((void**)&m->slab_tc, (size_t)tc_weight_floats(*cfg) * sizeof(float));
-    if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: cudaMalloc(tc weights) -> %s", cudaGetErrorString(e));
-    float* cur = m->slab_tc;
-#define TCPREP(src, K, N, dst) do { if (rc == MT3_OK) rc = prep_tc_weight(m, s, src, K, N, cur, dst); } while (0)
-    TCPREP(m->w_in, cfg->input_depth, D, &m->t_w_in);
-    for (int i = 0; i < m->Le; ++i) {
-      EncLayer& L = m->enc[i];
-      TCPREP(L.wqkv, D, 3 * Q, &L.t_wqkv);
-      TCPREP(L.wo, Q, D, &L.t_wo);
-      TCPREP(L.wi, D, 2 * F, &L.t_wi);
-      TCPREP(L.wo2, F, D, &L.t_wo2);
-    }
-    for (int i = 0; i < m->Ld; ++i) TCPREP(m->dec[i].wkv_c, D, 2 * Q, &m->dec[i].t_wkv_c);
-#undef TCPREP
-    if (rc == MT3_OK) {
-      e = cudaStreamSynchronize(s);
-      if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: tc weight prep -> %s", cudaGetErrorString(e));
-    }
-  }
+  if (rc == MT3_OK && m->tc)
+    rc = make_slab(&m->slab_tc, "mt3_model_create: tc weight prep", s, [&](Carve& c) -> int {
+      MT3_TRY(prep_tc_weight(m, s, m->w_in, cfg->input_depth, D, c, &m->t_w_in));
+      for (EncLayer& L : m->enc) {
+        MT3_TRY(prep_tc_weight(m, s, L.wqkv, D, 3 * Q, c, &L.t_wqkv));
+        MT3_TRY(prep_tc_weight(m, s, L.wo, Q, D, c, &L.t_wo));
+        MT3_TRY(prep_tc_weight(m, s, L.wi, D, 2 * F, c, &L.t_wi));
+        MT3_TRY(prep_tc_weight(m, s, L.wo2, F, D, c, &L.t_wo2));
+      }
+      for (DecLayer& L : m->dec) MT3_TRY(prep_tc_weight(m, s, L.wkv_c, D, 2 * Q, c, &L.t_wkv_c));
+      return MT3_OK;
+    });
   if (rc == MT3_OK) {
-    e = cudaMallocHost((void**)&m->h_flag, 4 * sizeof(int));
+    const cudaError_t e = cudaMallocHost((void**)&m->h_flag, 4 * sizeof(int));
     if (e != cudaSuccess) rc = fail(MT3_ERR_CUDA, "mt3_model_create: cudaMallocHost -> %s", cudaGetErrorString(e));
   }
   if (rc != MT3_OK) {
@@ -971,67 +1002,47 @@ extern "C" int mt3_model_destroy(mt3_model* h) {
   return MT3_OK;
 }
 
-namespace {
-struct WsLayout {
-  int64_t x_hi, x_lo, h_lo, ao_lo, g_lo, enc_hi, enc_lo, qkv_lo, vt_hi, vt_lo;
-  int64_t dy2, dssq;
-  int64_t h, rstd, qkv, ao, g, encoded, ckv, skv, dy, drstd, dq, dao, dg, dlogits, tok_cur, finished, tokens, state, dpartial, dcounters, beam_f, beam_i, att_scratch;
-  int64_t tok_scores, seq_scores, plen, prompt_info, pf_tok, total;
-};
-WsLayout ws_layout(const Model* m, int B, int T) {
-  WsLayout w;
-  int64_t off = 0;
-  auto take = [&](int64_t bytes) { int64_t r = off; off += align_up(bytes, 256); return r; };
-  const int64_t M = (int64_t)B * T, D = m->D, Q = m->Q, F = m->F, V = m->V, L = m->L;
-  const bool s3 = m->split3;
-  w.x_hi = take(s3 ? M * m->cfg.input_depth * 4 : 0);
-  w.x_lo = take(s3 ? M * m->cfg.input_depth * 4 : 0);
-  w.h_lo = take(s3 ? M * D * 4 : 0);
-  w.ao_lo = take(s3 ? M * Q * 4 : 0);
-  w.g_lo = take(s3 ? M * F * 4 : 0);
-  w.enc_hi = take(s3 ? M * D * 4 : 0);
-  w.enc_lo = take(s3 ? M * D * 4 : 0);
-  w.qkv_lo = take(s3 ? M * 3 * Q * 4 : 0);
-  w.vt_hi = take(m->tc ? M * Q * 4 : 0);
-  w.vt_lo = take(s3 ? M * Q * 4 : 0);
-  w.h = take(M * D * 4);
-  w.rstd = take(M * 4);
-  w.qkv = take(M * 3 * Q * 4);
-  w.ao = take(M * Q * 4);
-  w.g = take(M * F * 4);
-  w.encoded = take(M * D * 4);
-  w.ckv = take((int64_t)m->Ld * M * 2 * m->H * m->kv_row);
-  w.skv = take((int64_t)m->Ld * B * L * 2 * m->H * m->kv_row);
-  w.dy = take((int64_t)B * D * 4);
-  w.drstd = take((int64_t)B * 4);
-  w.dy2 = take((int64_t)B * D * 4);
-  w.dssq = take((int64_t)B * (D / 32) * 4);
-  w.dq = take((int64_t)B * Q * 4);
-  w.dao = take((int64_t)B * Q * 4);
-  w.dg = take((int64_t)B * F * 4);
-  w.dlogits = take((int64_t)B * V * 4);
-  w.tok_cur = take((int64_t)B * 4);
-  w.finished = take((int64_t)B * 4);
-  w.tokens = take((int64_t)B * L * 4);
-  w.state = take(64);
-  w.dpartial = take((int64_t)16 * cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * kDecTileFloats * 4);   // up to 16 K chunks
-  w.dcounters = take((int64_t)cdiv(std::max(std::max(3 * (int)Q, 2 * (int)F), (int)V), kDecBN) * 4);
-  w.att_scratch = take(m->tc ? attention_tc_scratch_floats(B, T, T, m->H, false) * 4 : 0);
-  w.beam_f = take((int64_t)B * 3 * 4);      // {live_lp, finished score} per sequence, then fin_lp_eos [B]
-  w.beam_i = take((int64_t)B * 4);
-  w.tok_scores = take((int64_t)B * L * 4);
-  w.seq_scores = take((int64_t)B * 4);
-  w.plen = take((int64_t)B * 4);
-  w.prompt_info = take(2 * 4);
-  w.pf_tok = take((int64_t)2 * B * L * 4);
-  w.total = off;
-  return w;
+// The model workspace for B sequences of T inputs
+static int carve_workspace(const Model* m, Carve& c, int B, int T, WsBuffers* w) {
+  const int64_t M = (int64_t)B * T, D = m->D, Q = m->Q, F = m->F, L = m->L;
+  MT3_TRY(carve_seq(m, c, B, T, false, 0, &w->ea));
+  if (m->split3) {
+    MT3_TRY(carve_act(m, c, M, m->cfg.input_depth, true, &w->a_x));
+    MT3_TRY(carve_act(m, c, M, m->D, true, &w->a_enc));
+  }
+  w->encoded = c.take(M * D);
+  w->ckv = c.take<char>((int64_t)m->Ld * M * 2 * m->H * m->kv_row);
+  w->skv = c.take<char>((int64_t)m->Ld * B * L * 2 * m->H * m->kv_row);
+  w->dy = c.take(B * D);
+  w->dy2 = c.take(B * D);
+  w->dssq = c.take(B * (D / 32));
+  w->dq = c.take(B * Q);
+  w->dao = c.take(B * Q);
+  w->dg = c.take(B * F);
+  w->dlogits = c.take((int64_t)B * m->V);
+  w->tok_cur = c.take<int>(B);
+  w->finished = c.take<int>(B);
+  w->tokens = c.take<int>(B * L);
+  w->state = c.take<int>(16);
+  w->dpartial = c.take((int64_t)16 * dec_tiles(m) * kDecTileFloats);   // up to 16 K chunks
+  w->dcounters = c.take<int>(dec_tiles(m));
+  w->beam_f = c.take(3 * B);      // {live_lp, finished score} per sequence, then fin_lp_eos [B]
+  w->fin_lp_eos = w->beam_f ? w->beam_f + 2 * B : nullptr;
+  w->beam_i = c.take<int>(B);
+  w->tok_scores = c.take(B * L);
+  w->seq_scores = c.take(B);
+  w->plen = c.take<int>(B);
+  w->prompt_info = c.take<int>(2);
+  w->pf_tok = c.take<int>(2 * B * L);
+  return MT3_OK;
 }
-}  // namespace
 
 extern "C" int64_t mt3_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length) {
   if (!h || batch <= 0 || input_length <= 0) return -1;
-  return ws_layout(reinterpret_cast<const Model*>(h), batch, input_length).total;
+  Carve c;
+  WsBuffers w;
+  carve_workspace(reinterpret_cast<const Model*>(h), c, batch, input_length, &w);
+  return c.used;
 }
 
 extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t bytes, int32_t batch, int32_t input_length) {
@@ -1041,37 +1052,14 @@ extern "C" int mt3_model_set_workspace(mt3_model* h, void* workspace, int64_t by
   MT3_REQUIRE(input_length > 0 && input_length <= m->cfg.max_input_length, MT3_ERR_SHAPE,
               "input_length %d outside (0, max_input_length=%d]", input_length, m->cfg.max_input_length);
   MT3_REQUIRE(((uintptr_t)workspace & 255) == 0, MT3_ERR_WORKSPACE, "workspace must be 256-byte aligned");
-  const WsLayout w = ws_layout(m, batch, input_length);
-  MT3_REQUIRE(bytes >= w.total, MT3_ERR_WORKSPACE, "workspace has %lld bytes, %lld needed", (long long)bytes, (long long)w.total);
-  char* b = (char*)workspace;
-  m->ws = b; m->ws_bytes = bytes; m->B = batch; m->T = input_length;
-  select_graph(m);
-  m->h = (float*)(b + w.h); m->rstd = (float*)(b + w.rstd); m->qkv = (float*)(b + w.qkv); m->ao = (float*)(b + w.ao);
-  m->g = (float*)(b + w.g); m->encoded = (float*)(b + w.encoded); m->ckv = b + w.ckv; m->skv = b + w.skv;
-  m->dy2 = (float*)(b + w.dy2); m->dssq = (float*)(b + w.dssq);
-  m->dy = (float*)(b + w.dy); m->drstd = (float*)(b + w.drstd); m->dq = (float*)(b + w.dq); m->dao = (float*)(b + w.dao);
-  m->dg = (float*)(b + w.dg); m->dlogits = (float*)(b + w.dlogits); m->tok_cur = (int*)(b + w.tok_cur);
-  m->finished = (int*)(b + w.finished); m->tokens = (int*)(b + w.tokens); m->state = (int*)(b + w.state);
-  m->dpartial = (float*)(b + w.dpartial); m->dcounters = (int*)(b + w.dcounters);
-  m->beam_f = (float*)(b + w.beam_f); m->beam_i = (int*)(b + w.beam_i); m->fin_lp_eos = m->beam_f + 2 * batch;
-  m->tok_scores = (float*)(b + w.tok_scores); m->seq_scores = (float*)(b + w.seq_scores);
-  m->plen = (int*)(b + w.plen); m->prompt_info = (int*)(b + w.prompt_info); m->pf_tok = (int*)(b + w.pf_tok);
-  const bool key_split = m->tc && attention_tc_scratch_floats(batch, input_length, input_length, m->H, false) > 0;
-  m->att_scratch = key_split ? (float*)(b + w.att_scratch) : nullptr;
-  m->dcounters_n = cdiv(std::max(std::max(3 * m->Q, 2 * m->F), m->V), kDecBN);
+  Carve c{(char*)workspace};
+  WsBuffers w;
+  MT3_TRY(carve_workspace(m, c, batch, input_length, &w));
+  MT3_REQUIRE(bytes >= c.used, MT3_ERR_WORKSPACE, "workspace has %lld bytes, %lld needed", (long long)bytes, (long long)c.used);
+  static_cast<WsBuffers&>(*m) = w;
+  m->ws = (char*)workspace; m->B = batch; m->T = input_length;
   m->have_cross = false;
-  const int64_t M = (int64_t)batch * input_length;
-  auto lo = [&](int64_t off) { return m->split3 ? (float*)(b + off) : nullptr; };
-  MT3_TRY(make_act(m, m->h, lo(w.h_lo), M, m->D, &m->a_h));
-  MT3_TRY(make_act(m, m->ao, lo(w.ao_lo), M, m->Q, &m->a_ao));
-  MT3_TRY(make_act(m, m->g, lo(w.g_lo), M, m->F, &m->a_g));
-  MT3_TRY(make_act(m, m->qkv, lo(w.qkv_lo), M, 3 * m->Q, &m->a_qkv));
-  if (m->split3) {
-    MT3_TRY(make_act(m, (float*)(b + w.x_hi), lo(w.x_lo), M, m->cfg.input_depth, &m->a_x));
-    MT3_TRY(make_act(m, (float*)(b + w.enc_hi), lo(w.enc_lo), M, m->D, &m->a_enc));
-  }
-  if (m->tc && input_length % 4 == 0)   // TMA row pitch must be a multiple of 16 bytes; otherwise the SIMT attention kernel runs
-    MT3_TRY(make_act(m, (float*)(b + w.vt_hi), lo(w.vt_lo), (int64_t)batch * m->H * 64, input_length, &m->a_vt, 64));
+  select_graph(m);
   return MT3_OK;
 }
 
@@ -1155,13 +1143,6 @@ __global__ void prefill_inputs_kernel(const int* __restrict__ prompt, int prompt
 // configuration (DESIGN.md §6): the pass over P <= 128 positions costs about as much as the loop's first 17 steps.
 constexpr int kPrefillMinP = 20;
 
-// Whether the teacher-forced pass can prefill P positions: the exact-fp32 attention kernel's limits where it runs
-static bool prefill_supported(const Model* m, int P) {
-  const int Lp = tf_pad(P);
-  return (tc_attention(m, Lp, Lp, true) || attention_fp32_smem(Lp) <= kAttFp32MaxSmem) &&
-         (tc_attention(m, Lp, m->T, false) || attention_fp32_smem(m->T) <= kAttFp32MaxSmem);
-}
-
 // mt3_generate, mt3_generate_scored and mt3_generate_prompted; `name` is the entry point the caller used, for its error
 // messages.  prompt_len == 0: no prompt (prompt and workspace unused).
 static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
@@ -1177,13 +1158,7 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
   MT3_REQUIRE(prompt_len >= 0 && prompt_len <= num_steps, MT3_ERR_BAD_ARG, "%s: prompt_len %d outside [0, num_steps=%d]", name, prompt_len,
               num_steps);
   MT3_REQUIRE(prompt_len == 0 || prompt, MT3_ERR_BAD_ARG, "%s: prompt is NULL with prompt_len %d", name, prompt_len);
-  if (prompt_len > 0) {
-    MT3_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, MT3_ERR_WORKSPACE,
-                "%s: the teacher-forced workspace must be non-null and 256-byte aligned when prompt_len > 0", name);
-    const int64_t need = tf_layout(m, m->B, m->T, prompt_len).total;
-    MT3_REQUIRE(workspace_bytes >= need, MT3_ERR_WORKSPACE, "%s: workspace has %lld bytes, %lld needed", name, (long long)workspace_bytes,
-                (long long)need);
-  }
+  if (prompt_len > 0) MT3_TRY(check_tf_workspace(m, name, workspace, workspace_bytes, m->B, m->T, prompt_len));
   cudaStream_t s = (cudaStream_t)stream;
   MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
@@ -1216,8 +1191,8 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
   // the shared prefix: one teacher-forced pass writes its K/V rows into the cache, and the loop starts at position P.
   // The tokens there are forced (plen), so they score 0 and finish nothing, as the loop's forced steps do.
   int start = 0;
-  if (P >= kPrefillMinP && prefill_supported(m, P)) {
-    MT3_REQUIRE(tf_layout(m, m->B, m->T, P).total <= workspace_bytes, MT3_ERR_WORKSPACE, "%s: workspace too small for the prefill", name);
+  if (P >= kPrefillMinP && tf_supported(m, m->T, P)) {
+    MT3_TRY(check_tf_workspace(m, name, workspace, workspace_bytes, m->B, m->T, P));
     MT3_TRY(ensure_tf_weights(m, s));
     int* dec_in = m->pf_tok;
     int* tgt = m->pf_tok + (int64_t)m->B * P;
@@ -1302,7 +1277,7 @@ extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_
   if (batch <= 0 || batch > m->cfg.max_batch || input_length <= 0 || input_length > m->cfg.max_input_length || target_length <= 0 ||
       target_length > m->L)
     return -1;
-  return tf_layout(m, batch, input_length, target_length).total;
+  return tf_workspace_bytes(m, batch, input_length, target_length);
 }
 
 extern "C" int mt3_decode_teacher_forced(mt3_model* h, const float* encoded, int32_t batch, int32_t input_length,
@@ -1318,16 +1293,11 @@ extern "C" int mt3_decode_teacher_forced(mt3_model* h, const float* encoded, int
               "input_length %d outside (0, max_input_length=%d]", input_length, m->cfg.max_input_length);
   MT3_REQUIRE(target_length > 0 && target_length <= m->L, MT3_ERR_SHAPE, "target_length %d outside (0, max_decode_length=%d]",
               target_length, m->L);
-  MT3_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, MT3_ERR_WORKSPACE, "workspace must be non-null and 256-byte aligned");
-  const TfLayout w = tf_layout(m, batch, input_length, target_length);
-  MT3_REQUIRE(workspace_bytes >= w.total, MT3_ERR_WORKSPACE, "workspace has %lld bytes, %lld needed", (long long)workspace_bytes,
-              (long long)w.total);
-  // the exact-fp32 attention kernel's limit where it runs, and the wgmma GEMM's N tiling of the logits projection
-  const int Lp = tf_pad(target_length);
-  MT3_REQUIRE(tc_attention(m, Lp, Lp, true) || attention_fp32_smem(Lp) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED,
-              "mt3_decode_teacher_forced: target_length %d too long for the exact-fp32 attention kernel", target_length);
-  MT3_REQUIRE(tc_attention(m, Lp, input_length, false) || attention_fp32_smem(input_length) <= kAttFp32MaxSmem, MT3_ERR_UNSUPPORTED,
-              "mt3_decode_teacher_forced: input_length %d too long for the exact-fp32 attention kernel", input_length);
+  MT3_TRY(check_tf_workspace(m, "mt3_decode_teacher_forced", workspace, workspace_bytes, batch, input_length, target_length));
+  MT3_REQUIRE(tf_supported(m, input_length, target_length), MT3_ERR_UNSUPPORTED,
+              "mt3_decode_teacher_forced: target_length %d or input_length %d too long for the exact-fp32 attention kernel", target_length,
+              input_length);
+  // the wgmma GEMM's N tiling of the logits projection
   MT3_REQUIRE(!m->tc || m->V % 32 == 0, MT3_ERR_UNSUPPORTED, "mt3_decode_teacher_forced: the wgmma logits GEMM needs vocab %% 32 == 0");
   cudaStream_t s = (cudaStream_t)stream;
   MT3_TRY(ensure_tf_weights(m, s));
@@ -1437,16 +1407,16 @@ extern "C" int mt3_debug_launch(mt3_model* h, int32_t kind, int32_t pos, int32_t
       case MT3_K_DEC_QKV_GEMM: {
         // scratch output: the encoder qkv buffer (B*T rows >= B).  Not the cache: after a full generate, *state is
         // max_decode_length, and an append there would write past it.
-        MT3_TRY(dec_gemm(m, "gemm_qkv", m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->qkv, 3 * Q, 3 * Q, nullptr, nullptr, s));
+        MT3_TRY(dec_gemm(m, "gemm_qkv", m->dy, D, m->dec[l].wqkv, 3 * Q, D, 1, EPI_STORE, m->ea.qkv.hi, 3 * Q, 3 * Q, nullptr, nullptr, s));
         break;
       }
       case MT3_K_ENC_QKV_GEMM: {
         const EncLayer& w = m->enc[it % std::max(1, m->Le)];
-        MT3_TRY(seq_qkv(m, m->a_h, m->B * T, m->rstd, w.wqkv, w.t_wqkv, m->a_qkv, enc_vt(m), T, s));
+        MT3_TRY(seq_qkv(m, m->ea, w.wqkv, w.t_wqkv, s));
         break;
       }
       case MT3_K_ENC_ATTN: {
-        MT3_TRY(seq_self_attention(m, m->a_qkv, enc_vt(m), m->B, T, nullptr, 0, false, m->a_ao, m->att_scratch, s));
+        MT3_TRY(seq_self_attention(m, m->ea, nullptr, 0, false, s));
         break;
       }
       default:

@@ -97,6 +97,16 @@ class Transformer:
         _lib.check(self._lib.mt3_model_set_workspace(self._h, self._ws.data_ptr(), self._ws.numel(), batch, length))
         self._ws_key = key
 
+    def _tf_workspace(self, batch: int, input_length: int, length: int) -> torch.Tensor:
+        """The teacher-forced pass's workspace for `length` targets, grown when it is too small."""
+        nbytes = int(self._lib.mt3_teacher_forced_workspace_bytes(self._h, batch, input_length, length))
+        if nbytes <= 0:
+            raise _lib.Mt3Error(-2, f"no teacher-forced workspace layout for batch={batch}, input_length={input_length}, length={length}")
+        if self._tf_ws is None or self._tf_ws.numel() < nbytes:
+            self._tf_ws = None
+            self._tf_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self._tf_ws
+
     def _check_inputs(self, x: torch.Tensor):
         if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32):
             raise TypeError("encoder_input_tokens must be a CUDA float32 tensor")
@@ -218,12 +228,7 @@ class Transformer:
             lo, hi = int(x.min()), int(x.max())
             if lo < 0 or hi >= v:
                 raise ValueError(f'{name}: ids must lie in [0, vocab_size={v}); got [{lo}, {hi}]')
-        nbytes = int(self._lib.mt3_teacher_forced_workspace_bytes(self._h, b, t, length))
-        if nbytes <= 0:
-            raise _lib.Mt3Error(-2, f"no teacher-forced workspace layout for batch={b}, input_length={t}, length={length}")
-        if self._tf_ws is None or self._tf_ws.numel() < nbytes:
-            self._tf_ws = None
-            self._tf_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self._tf_workspace(b, t, length)
         logits = torch.empty((b, length, v), dtype=torch.float32, device=self.device) if want_logits else None
         scores = torch.empty((b, length), dtype=torch.float32, device=self.device) if want_scores else None
         enc = encoded.contiguous()
@@ -231,7 +236,7 @@ class Transformer:
             _lib.check(self._lib.mt3_decode_teacher_forced(
                 self._h, enc.data_ptr(), b, t, tok_in.data_ptr(), tgt.data_ptr(), None if wts is None else wts.data_ptr(), length,
                 None if logits is None else logits.data_ptr(), None if scores is None else scores.data_ptr(),
-                self._tf_ws.data_ptr(), self._tf_ws.numel(), self._stream()))
+                ws.data_ptr(), ws.numel(), self._stream()))
         return logits, scores
 
     # -- helpers built on the step ----------------------------------------------------
@@ -304,12 +309,7 @@ class Transformer:
 
     def _generate_prompted(self, x, steps: int, flags: int, prompt: torch.Tensor, out: torch.Tensor, return_scores: bool):
         b, t, _ = x.shape
-        nbytes = int(self._lib.mt3_teacher_forced_workspace_bytes(self._h, b, t, prompt.shape[1]))
-        if nbytes <= 0:
-            raise _lib.Mt3Error(-2, f"no teacher-forced workspace layout for batch={b}, input_length={t}, length={prompt.shape[1]}")
-        if self._tf_ws is None or self._tf_ws.numel() < nbytes:
-            self._tf_ws = None
-            self._tf_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self._tf_workspace(b, t, prompt.shape[1])
         token_scores = torch.empty((b, self.max_decode_length), dtype=torch.float32, device=self.device) if return_scores else None
         scores = torch.empty((b,), dtype=torch.float32, device=self.device) if return_scores else None
         ran = C.c_int32(0)
@@ -317,6 +317,6 @@ class Transformer:
             _lib.check(self._lib.mt3_generate_prompted(
                 self._h, x.data_ptr(), steps, flags, prompt.data_ptr(), prompt.shape[1], out.data_ptr(),
                 None if token_scores is None else token_scores.data_ptr(), None if scores is None else scores.data_ptr(), C.byref(ran),
-                self._tf_ws.data_ptr(), self._tf_ws.numel(), self._stream()))
+                ws.data_ptr(), ws.numel(), self._stream()))
         self.last_steps_run = int(ran.value)
         return (out, token_scores, scores) if return_scores else out
