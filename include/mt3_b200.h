@@ -19,7 +19,8 @@
  *     reference's fail-fast Python exceptions (rank asserts network.py:53,168,211,
  *     281; cache shape ValueError layers.py:266-270; bad token dtype layers.py:528).
  *   - handles are not thread-safe; one host thread per GPU/process.
- *   - inference only: dropout off, no RNG (deterministic=True paths).
+ *   - inference only: dropout off.  The one random stream is the sampling picker's (mt3_generate_sampled):
+ *     counter-based (Philox4x32-10), so a result depends on the key, the row's stream index and the position only.
  */
 #ifndef MT3_B200_H_
 #define MT3_B200_H_
@@ -165,11 +166,12 @@ int mt3_decode_step(mt3_model* m, const int32_t* tok_in, float* logits, int32_t*
 enum {
   MT3_GEN_STOP_AT_EOS = 1,   /* end the loop once every sequence emitted EOS (id 1)   */
   MT3_GEN_USE_GRAPH = 2,     /* replay one captured CUDA graph per step                */
-  MT3_GEN_BEAM1 = 4          /* t5x decoding.beam_search bookkeeping at num_decodes = 1 (the reference's decode_fn,
+  MT3_GEN_BEAM1 = 4,         /* t5x decoding.beam_search bookkeeping at num_decodes = 1 (the reference's decode_fn,
                                 models.py:127) instead of greedy-until-EOS: the live prefix continues with the best non-EOS
                                 token, "prefix + EOS" hypotheses are ranked by log-prob / ((5 + length) / 6)^0.6, and the best
                                 finished hypothesis is returned.  With MT3_GEN_STOP_AT_EOS the loop ends once every sequence's
                                 finished score beats what its live prefix can still reach.                                */
+  MT3_GEN_SAMPLE = 8         /* t5x decoding.temperature_sample's pick (mt3_generate_sampled only); not with MT3_GEN_BEAM1   */
 };
 
 /* predict_batch_with_aux stand-in (models.py:121-138 + t5x decode loop, greedy):
@@ -240,6 +242,36 @@ int mt3_decode_teacher_forced(mt3_model* m, const float* encoded, int32_t batch,
 int mt3_generate_prompted(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt, int32_t prompt_len,
                           int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run, void* workspace,
                           int64_t workspace_bytes, void* stream);
+
+/* Sampling parameters of mt3_generate_sampled.
+ *   temperature: z = logits / temperature (float32 division), finite and >= 0.  At or below 1e-4 the greedy loop runs
+ *     unchanged (T5X's MIN_TEMPERATURE): the tokens and scores of mt3_generate_prompted, bit for bit.
+ *   topk: 0 = off; else keep every id whose z is >= the k-th largest z (ties kept); topk >= vocab keeps all.
+ *   topp: 0 or 1 = off; else, after top-k, keep id i iff the softmax mass of the kept ids with z_j > z_i is below topp.
+ *   top-k and top-p need vocab_size <= 4096 (MT3_ERR_UNSUPPORTED otherwise).
+ *   key: the 64-bit Philox key (a JAX PRNGKey's two words as they are).  row0: row b draws from stream row0 + b.
+ *   rescale_log_probs: != 0, token scores are log-probabilities under the distribution sampled from,
+ *     z[next] - logsumexp(kept z) (T5X's default); 0, logits[next] - logsumexp(logits row), as greedy's. */
+typedef struct mt3_sample_params {
+  float temperature;
+  int32_t topk;
+  float topp;
+  uint32_t key[2];
+  uint32_t row0;
+  int32_t rescale_log_probs;
+} mt3_sample_params;
+
+/* mt3_generate_prompted with flags | MT3_GEN_SAMPLE: each free position draws its token from the filtered softmax of
+ * z by the Gumbel-max rule, next = argmax_i (z_i - log(-log(u_i))) over the kept ids (the first id wins a tie), with
+ * u_i from Philox4x32-10 at counter (i / 4, position, row0 + b, 0), word i % 4, mapped to (2 (w >> 9) + 1) 2^-24.  The
+ * numbers of a row depend only on (key, row0 + b, position): not on graphs, early stop, prefill or batch size.
+ * EOS, PAD, NaN rows, forced prompt positions and scores_out (the sum of the token scores) are greedy's.
+ * params HOST (required with MT3_GEN_SAMPLE, MT3_ERR_BAD_ARG otherwise, as are a temperature that is not finite and
+ * >= 0, topk < 0, topp outside [0, 1] and MT3_GEN_SAMPLE | MT3_GEN_BEAM1).  Without MT3_GEN_SAMPLE this is
+ * mt3_generate_prompted.  Synchronises the stream once to copy params. */
+int mt3_generate_sampled(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt, int32_t prompt_len,
+                         int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run, void* workspace,
+                         int64_t workspace_bytes, const mt3_sample_params* params, void* stream);
 
 /* GenericTokenVocabulary._decode_tf (vocabularies.py:241-271): ids DEV i32 [B, L]
  * -> out DEV i32 [B, L] with id-3, EOS-and-after = -1, invalid = -2. */

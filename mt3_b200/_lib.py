@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(HERE, "libmt3b200.so")
 MT3_OK = 0
 GEMM_FP32_SIMT, GEMM_TF32X3, GEMM_TF32 = 0, 1, 2
 KV_F32, KV_F16, KV_P24 = 0, 1, 2
-GEN_STOP_AT_EOS, GEN_USE_GRAPH, GEN_BEAM1 = 1, 2, 4
+GEN_STOP_AT_EOS, GEN_USE_GRAPH, GEN_BEAM1, GEN_SAMPLE = 1, 2, 4, 8
 ABI_VERSION = 2
 K_DEC_SELF_ATTN, K_DEC_CROSS_ATTN, K_DEC_QKV_GEMM, K_ENC_QKV_GEMM, K_ENC_ATTN = 0, 1, 2, 3, 4
 
@@ -25,7 +25,7 @@ EXPORTS = [
     "mt3_model_num_params", "mt3_model_param_offset", "mt3_model_create", "mt3_model_destroy",
     "mt3_workspace_bytes", "mt3_model_set_workspace", "mt3_encode", "mt3_cross_kv", "mt3_decode_step",
     "mt3_generate", "mt3_generate_scored", "mt3_vocab_decode", "mt3_dot_product_attention_f32", "mt3_debug_launch", "mt3_debug_trace_step",
-    "mt3_teacher_forced_workspace_bytes", "mt3_decode_teacher_forced", "mt3_generate_prompted",
+    "mt3_teacher_forced_workspace_bytes", "mt3_decode_teacher_forced", "mt3_generate_prompted", "mt3_generate_sampled",
 ]
 
 
@@ -46,6 +46,11 @@ class ModelConfig(C.Structure):
                 ("mlp_dim", C.c_int32), ("input_depth", C.c_int32), ("max_batch", C.c_int32),
                 ("max_input_length", C.c_int32), ("max_decode_length", C.c_int32), ("gemm_mode", C.c_int32),
                 ("kv_cache_format", C.c_int32)]
+
+
+class SampleParams(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("topk", C.c_int32), ("topp", C.c_float), ("key", C.c_uint32 * 2),
+                ("row0", C.c_uint32), ("rescale_log_probs", C.c_int32)]
 
 
 _lib = None
@@ -84,6 +89,8 @@ def load() -> C.CDLL:
     lib.mt3_generate.argtypes = [vp, f32p, i32, i32, i32p, C.POINTER(i32), vp]
     lib.mt3_generate_scored.argtypes = [vp, f32p, i32, i32, i32p, f32p, f32p, C.POINTER(i32), vp]
     lib.mt3_generate_prompted.argtypes = [vp, f32p, i32, i32, i32p, i32, i32p, f32p, f32p, C.POINTER(i32), vp, i64, vp]
+    lib.mt3_generate_sampled.argtypes = [vp, f32p, i32, i32, i32p, i32, i32p, f32p, f32p, C.POINTER(i32), vp, i64,
+                                         C.POINTER(SampleParams), vp]
     lib.mt3_vocab_decode.argtypes = [i32p, i32, i32, i32, i32p, vp]
     lib.mt3_dot_product_attention_f32.argtypes = [f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p, vp]
     lib.mt3_debug_launch.argtypes = [vp, i32, i32, i32, vp]

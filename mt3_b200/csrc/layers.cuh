@@ -4,6 +4,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace mt3 {
 
@@ -590,6 +591,224 @@ __global__ void __launch_bounds__(128) seq_score_kernel(const float* __restrict_
 
 inline int launch_seq_score(const float* token_scores, int B, int L, float* scores, cudaStream_t s) {
   seq_score_kernel<<<B, 128, 0, s>>>(token_scores, L, scores);
+  MT3_LAUNCH_CHECK();
+  return MT3_OK;
+}
+
+// ---------------------------------------------------------------------------------
+// T5X decoding.temperature_sample's pick (mt3_generate_sampled), one CTA per sequence, parameters from sp (device):
+//   z = logits / temperature (IEEE division), kept in shared memory;
+//   top-k (0 < topk < V): keep every id whose z is >= the k-th largest z (ties at the k-th value are all kept);
+//   top-p (0 < topp < 1), after top-k: keep id i iff the softmax mass of the kept ids with z_j > z_i is below topp;
+//   next = argmax_i (z_i + g_i) over the kept ids (the first id wins a tie), g_i = -log(-log(u_i)), u_i from
+//     Philox4x32-10 with key sp->key and counter (i / 4, pos, sp->row0 + b, 0), word i % 4 (philox.cuh): a row's
+//     numbers depend only on (key, stream, position).
+// The filters sort (order-preserving key of z, id) pairs, V padded to a power of two (nsort), with a bitonic network in
+// shared memory, then cut the sorted row at the k-th value and at the first tie group whose preceding mass, summed in one
+// fixed order, reaches topp: both cuts are deterministic.  The dropped ids become -inf in the z row.
+// token_scores: sp->rescale_log_probs != 0: z[next] - logsumexp(kept z); else logits[next] - logsumexp(logits row), greedy's
+// bits.  Both through block_logsumexp.  A row with a NaN emits its first NaN id with a NaN score, as argmax_step_kernel.
+// The bookkeeping (finished rows emit PAD with score 0, EOS finishes, forced prompt positions, the arrival counter that
+// advances state, y_next) is argmax_step_kernel's.
+// ---------------------------------------------------------------------------------
+constexpr int kSampleMaxSortV = 4096;          // the largest vocabulary the top-k / top-p filters sort
+constexpr int kSampleMaxSmem = 200 * 1024;
+
+// nsort: the sort's padded length (0 when V is too large to sort); the dynamic shared memory is nsort pairs and the z row
+inline int sample_sort_n(int V) {
+  if (V > kSampleMaxSortV) return 0;
+  int n = 256;
+  while (n < V) n <<= 1;
+  return n;
+}
+inline size_t sample_step_smem(int V) { return (size_t)sample_sort_n(V) * 8 + (size_t)V * 4; }
+
+// ascending in the result = descending in z (-0.0 after +0.0; NaN never reaches the sort)
+__device__ __forceinline__ uint32_t z_order_desc(float z) {
+  const uint32_t u = __float_as_uint(z);
+  return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
+}
+
+__global__ void __launch_bounds__(256)
+sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, int* __restrict__ tok_cur, int* __restrict__ finished,
+                   int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                   int* __restrict__ state, const mt3_sample_params* __restrict__ sp, const float* __restrict__ emb,
+                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  unsigned long long* skey = reinterpret_cast<unsigned long long*>(smem_raw);   // [nsort] (z order << 32 | id)
+  float* z = reinterpret_cast<float*>(smem_raw + (size_t)nsort * 8);              // [V]
+  __shared__ float sv[8], slse[8], sscan[8];
+  __shared__ int si[8], snan[8];
+  __shared__ int s_cut[2];
+  __shared__ int s_next[2];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // plen and the parameters are written before the encoder runs: their loads go ahead of the wait
+  const int pl = (plen && tid == 0) ? plen[b] : 0;
+  const float temp = sp->temperature, topp = sp->topp;
+  const int topk = sp->topk, rescale = sp->rescale_log_probs;
+  const uint32_t k0 = sp->key[0], k1 = sp->key[1], stream = sp->row0 + (uint32_t)b;
+  pdl_wait();
+  pdl_trigger();
+  const float* l = logits + (long long)b * V;
+  // read by every thread before its CTA arrives at the counter (the barriers below), so before the last CTA advances it
+  const int pos = state[0];
+  int nan_i = 0x7fffffff;
+  for (int i = tid; i < V; i += 256) {
+    const float v = l[i];
+    z[i] = v / temp;
+    if (v != v) nan_i = min(nan_i, i);
+  }
+  nan_i = __reduce_min_sync(0xffffffffu, nan_i);
+  if (lane == 0) snan[warp] = nan_i;
+  if (tid == 0) { s_cut[0] = V; s_cut[1] = V; }
+  __syncthreads();
+#pragma unroll
+  for (int w = 0; w < 8; ++w) nan_i = min(nan_i, snan[w]);
+  const bool has_nan = nan_i != 0x7fffffff;
+  const bool use_k = topk > 0 && topk < V, use_p = topp > 0.f && topp < 1.f;
+  if (!has_nan && (use_k || use_p) && nsort >= V) {
+    for (int j = tid; j < nsort; j += 256)
+      skey[j] = j < V ? ((unsigned long long)z_order_desc(z[j]) << 32) | (unsigned)j : ~0ull;
+    __syncthreads();
+    for (int k = 2; k <= nsort; k <<= 1) {
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        for (int t = tid; t < nsort / 2; t += 256) {
+          const int i = 2 * t - (t & (j - 1)), p = i + j;
+          const unsigned long long a = skey[i], c = skey[p];
+          if ((a > c) == ((i & k) == 0)) { skey[i] = c; skey[p] = a; }
+        }
+        __syncthreads();
+      }
+    }
+    auto zs = [&](int j) { return z[(int)(skey[j] & 0xffffffffu)]; };
+    if (use_k) {     // the one sorted position where the run of values >= the k-th value ends
+      const float zk = zs(topk - 1);
+      for (int j = topk - 1 + tid; j < V; j += 256)
+        if (zs(j) >= zk && (j + 1 == V || zs(j + 1) < zk)) s_cut[0] = j + 1;
+      __syncthreads();
+    }
+    const int n1 = s_cut[0];
+    if (use_p) {
+      // thread t holds sorted positions [t c, t c + c): its sum in order, an exclusive scan of the 256 sums (warp shuffles,
+      // then the 8 warp totals in order), then its own positions again in order
+      const int c = nsort / 256;
+      const float z0 = zs(0);
+      float run = 0.f;
+      for (int q = 0; q < c; ++q) {
+        const int j = tid * c + q;
+        if (j < n1) run += expf(zs(j) - z0);
+      }
+      float incl = run;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const float y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+      }
+      float m = __shfl_up_sync(0xffffffffu, incl, 1);
+      if (lane == 0) m = 0.f;
+      if (lane == 31) sscan[warp] = incl;
+      __syncthreads();
+      float base = 0.f, tot = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) {
+        if (w == warp) base = tot;
+        tot += sscan[w];
+      }
+      m += base;
+      const float thr = topp * tot;
+      for (int q = 0; q < c; ++q) {
+        const int j = tid * c + q;
+        if (j >= n1) break;
+        const float zj = zs(j);
+        if (j > 0 && zj < zs(j - 1) && m >= thr) { atomicMin(&s_cut[1], j); break; }
+        m += expf(zj - z0);
+      }
+      __syncthreads();
+    }
+    // the kept ids are the sorted prefix [0, n): z >= its last value.  That id's z is kept, so no thread overwrites it.
+    const float zc = zs(min(n1, s_cut[1]) - 1);
+    for (int i = tid; i < V; i += 256)
+      if (!(z[i] >= zc)) z[i] = -INFINITY;
+    __syncthreads();
+  }
+  // Gumbel-max: thread t draws the ids 4 j .. 4 j + 3 of the Philox blocks j = t, t + 256, ...
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
+  if (!has_nan) {
+    for (int j = tid; 4 * j < V; j += 256) {
+      uint32_t w[4];
+      philox4x32_10((uint32_t)j, (uint32_t)pos, stream, 0u, k0, k1, w);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int i = 4 * j + q;
+        if (i < V) {
+          const float v = z[i] + (-logf(-logf(philox_uniform(w[q]))));
+          if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+  }
+  if (lane == 0) { sv[warp] = best; si[warp] = bi; }
+  __syncthreads();
+  const float lse = (token_scores && !has_nan) ? block_logsumexp(rescale ? z : l, V, slse) : 0.f;
+  if (tid == 0) {
+    for (int w = 1; w < 8; ++w)
+      if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
+    int nxt = has_nan ? nan_i : bi;
+    float lp = 0.f;
+    if (token_scores) lp = has_nan ? __int_as_float(0x7fffffff) : (rescale ? z[nxt] : l[nxt]) - lse;
+    if (pos < pl) {                       // forced: the prompt token (never EOS), so the sequence cannot finish here
+      nxt = tokens_out[(long long)b * out_ld + pos];
+      lp = 0.f;
+    } else {
+      if (finished[b]) { nxt = 0; lp = 0.f; }
+      if (nxt == 1) finished[b] = 1;
+    }
+    s_next[0] = nxt;
+    s_next[1] = pos + 1;
+    tok_cur[b] = nxt;
+    tokens_out[(long long)b * out_ld + pos] = nxt;
+    if (token_scores) token_scores[(long long)b * out_ld + pos] = lp;
+    __threadfence();
+    const int done = atomicAdd(&state[1], 1);
+    if (done == B - 1) {
+      __threadfence();
+      int all = 1;
+      for (int i = 0; i < B; ++i) all &= (*(volatile int*)&finished[i]) != 0;
+      state[2] = all;
+      state[1] = 0;
+      state[0] = pos + 1;
+    }
+  }
+  if (y_next) {
+    __syncthreads();
+    const int t = min(max(s_next[0], 0), V - 1), p1 = s_next[1];
+    if (p1 >= pe_rows) return;
+    const float4* e = reinterpret_cast<const float4*>(emb + (long long)t * D);
+    const float4* pp = reinterpret_cast<const float4*>(pe + (long long)p1 * D);
+    float4* o = reinterpret_cast<float4*>(y_next + (long long)b * D);
+    for (int i = tid; i < D / 4; i += 256) {
+      const float4 a = __ldg(e + i), c = __ldg(pp + i);
+      o[i] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
+    }
+  }
+}
+
+// every sequence of a batch of B; sp DEV.  Top-k / top-p at V > kSampleMaxSortV are refused by the caller, which knows sp.
+inline int launch_sample_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                              int out_ld, const int* plen, int* state, const mt3_sample_params* sp, const float* emb, const float* pe,
+                              int pe_rows, int D, float* y_next, cudaStream_t s) {
+  const size_t smem = sample_step_smem(V);
+  MT3_REQUIRE(smem <= (size_t)kSampleMaxSmem, MT3_ERR_UNSUPPORTED, "sampling: vocabulary %d too large for one CTA's row", V);
+  MT3_TRY(set_max_dynamic_smem<sample_step_kernel>(kSampleMaxSmem));
+  MT3_CUDA_CHECK(launch_kernel(sample_step_kernel, dim3(B), dim3(256), smem, s, false, logits, V, B, sample_sort_n(V), tok_cur, finished,
+                               tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }

@@ -126,6 +126,7 @@ struct WsBuffers {
   int* plen = nullptr;            // [B] forced prompt lengths of the token pickers (0 = free from position 0)
   int* prompt_info = nullptr;     // {P = shortest prompt, 1 + first invalid row or 0} of prompt_scan_kernel
   int* pf_tok = nullptr;          // [2][B, L] decoder inputs and key-validity targets of the prefill pass
+  mt3_sample_params* sample = nullptr;   // the sampling picker's parameters (MT3_GEN_SAMPLE), written once per generate
   float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
   int* dcounters = nullptr;       // [dec_tiles()]
 };
@@ -572,6 +573,9 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->beam_f,
                               m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, kPeRows, m->D, y_next, s));
+  } else if (greedy == 3) { // T5X temperature_sample's pick (generate loop only), parameters in the workspace
+    MT3_TRY(launch_sample_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->sample,
+                               m->emb, m->pe, kPeRows, m->D, y_next, s));
   } else if (greedy) {
     MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
                                tok_scores, m->L, loop_step ? m->plen : nullptr, tok_user, m->state, 1, 0, m->emb, m->pe, kPeRows, m->D,
@@ -604,7 +608,7 @@ static void select_graph(Model* m, int mode = 1) {
   }
 }
 
-// mode: 1 greedy, 2 beam-size-1 search; nsteps consecutive decode steps per graph (the position lives on the device, so a
+// mode: 1 greedy, 2 beam-size-1 search, 3 sampling; nsteps consecutive decode steps per graph (the position lives on the device, so a
 // graph of 16 steps is the single-step graph 16 times over: one graph launch and its ~3 us of inter-launch latency per 16 steps);
 // scored: the token pickers write token scores (a graph of its own, so that the unscored graphs do no extra work)
 static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
@@ -628,10 +632,10 @@ static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
   m->graph_kernels = g_launch_count.load() - before;
   g_launch_count.fetch_sub(m->graph_kernels);   // capture does not execute
   MT3_CUDA_CHECK(cudaGraphInstantiate(&m->graph_exec, m->graph, 0));
-  // bound the cache: forget the graphs of other (workspace, B, T) bindings.  The current binding's stay: it has at most 8
-  // (2 modes x scored or not x 1 or 16 steps), and a caller may still hold one of them (mt3_generate_scored keeps the
+  // bound the cache: forget the graphs of other (workspace, B, T) bindings.  The current binding's stay: it has at most 12
+  // (3 modes x scored or not x 1 or 16 steps), and a caller may still hold one of them (mt3_generate_scored keeps the
   // 16-step graph while it makes sure of the single-step one).
-  if (m->graphs.size() >= 12) {
+  if (m->graphs.size() >= 16) {
     for (auto it = m->graphs.begin(); it != m->graphs.end();) {
       if (std::get<0>(it->first) != (const void*)m->ws || std::get<1>(it->first) != m->B || std::get<2>(it->first) != m->T) {
         cudaGraphExecDestroy(it->second.e);
@@ -1034,6 +1038,7 @@ static int carve_workspace(const Model* m, Carve& c, int B, int T, WsBuffers* w)
   w->plen = c.take<int>(B);
   w->prompt_info = c.take<int>(2);
   w->pf_tok = c.take<int>(2 * B * L);
+  w->sample = c.take<mt3_sample_params>(1);
   return MT3_OK;
 }
 
@@ -1143,18 +1148,33 @@ __global__ void prefill_inputs_kernel(const int* __restrict__ prompt, int prompt
 // configuration (DESIGN.md §6): the pass over P <= 128 positions costs about as much as the loop's first 17 steps.
 constexpr int kPrefillMinP = 20;
 
-// mt3_generate, mt3_generate_scored and mt3_generate_prompted; `name` is the entry point the caller used, for its error
-// messages.  prompt_len == 0: no prompt (prompt and workspace unused).
+// Temperatures at or below this pick greedily (T5X's MIN_TEMPERATURE): MT3_GEN_SAMPLE then runs the greedy loop unchanged.
+constexpr float kMinTemperature = 1e-4f;
+
+// mt3_generate, mt3_generate_scored, mt3_generate_prompted and mt3_generate_sampled; `name` is the entry point the caller used,
+// for its error messages.  prompt_len == 0: no prompt (prompt and workspace unused).  sp: HOST, read with MT3_GEN_SAMPLE only.
 static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
                          int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run,
-                         void* workspace, int64_t workspace_bytes, void* stream) {
+                         void* workspace, int64_t workspace_bytes, const mt3_sample_params* sp, void* stream) {
   MT3_REQUIRE(h && x && tokens_out, MT3_ERR_BAD_ARG, "%s: null argument", name);
   Model* m = reinterpret_cast<Model*>(h);
   MT3_NEED_WS(m);
   MT3_REQUIRE(num_steps >= 0 && num_steps <= m->L, MT3_ERR_SHAPE, "%s: num_steps %d outside [0, max_decode_length=%d]", name, num_steps,
               m->L);
-  MT3_REQUIRE((flags & ~(MT3_GEN_STOP_AT_EOS | MT3_GEN_USE_GRAPH | MT3_GEN_BEAM1)) == 0, MT3_ERR_BAD_ARG, "%s: unknown flag bits 0x%x", name,
-              flags);
+  MT3_REQUIRE((flags & ~(MT3_GEN_STOP_AT_EOS | MT3_GEN_USE_GRAPH | MT3_GEN_BEAM1 | MT3_GEN_SAMPLE)) == 0, MT3_ERR_BAD_ARG,
+              "%s: unknown flag bits 0x%x", name, flags);
+  const bool sample = (flags & MT3_GEN_SAMPLE) != 0;
+  if (sample) {
+    MT3_REQUIRE(!(flags & MT3_GEN_BEAM1), MT3_ERR_BAD_ARG, "%s: MT3_GEN_SAMPLE and MT3_GEN_BEAM1 exclude each other", name);
+    MT3_REQUIRE(sp, MT3_ERR_BAD_ARG, "%s: MT3_GEN_SAMPLE without sampling parameters", name);
+    MT3_REQUIRE(isfinite(sp->temperature) && sp->temperature >= 0.f, MT3_ERR_BAD_ARG, "%s: temperature %g is not finite and >= 0", name,
+                (double)sp->temperature);
+    MT3_REQUIRE(sp->topk >= 0, MT3_ERR_BAD_ARG, "%s: topk %d < 0", name, sp->topk);
+    MT3_REQUIRE(sp->topp >= 0.f && sp->topp <= 1.f, MT3_ERR_BAD_ARG, "%s: topp %g outside [0, 1]", name, (double)sp->topp);
+  }
+  const bool filtered = sample && ((sp->topk > 0 && sp->topk < m->V) || (sp->topp > 0.f && sp->topp < 1.f));
+  MT3_REQUIRE(!filtered || m->V <= kSampleMaxSortV, MT3_ERR_UNSUPPORTED, "%s: top-k / top-p need vocab_size <= %d (have %d)", name,
+              kSampleMaxSortV, m->V);
   MT3_REQUIRE(prompt_len >= 0 && prompt_len <= num_steps, MT3_ERR_BAD_ARG, "%s: prompt_len %d outside [0, num_steps=%d]", name, prompt_len,
               num_steps);
   MT3_REQUIRE(prompt_len == 0 || prompt, MT3_ERR_BAD_ARG, "%s: prompt is NULL with prompt_len %d", name, prompt_len);
@@ -1162,6 +1182,11 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
   cudaStream_t s = (cudaStream_t)stream;
   MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
+  if (sample && sp->temperature > kMinTemperature) {
+    // one graph per (mode, scored, steps) serves every parameter set: the picker reads them from the workspace
+    MT3_CUDA_CHECK(cudaMemcpyAsync(m->sample, sp, sizeof(mt3_sample_params), cudaMemcpyHostToDevice, s));
+    MT3_CUDA_CHECK(cudaStreamSynchronize(s));        // `sp` is the caller's pageable memory
+  }
   int P = 0;                                    // prompt prefix every row shares
   if (prompt_len > 0) {
     prompt_scan_kernel<<<1, 256, 0, s>>>(prompt, m->B, prompt_len, m->V, m->plen, m->tokens, m->L, m->prompt_info);
@@ -1180,7 +1205,7 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
   if (scored) MT3_CUDA_CHECK(cudaMemsetAsync(m->tok_scores, 0, (size_t)m->B * m->L * sizeof(float), s));
   const bool use_graph = (flags & MT3_GEN_USE_GRAPH) != 0;
   const bool stop = (flags & MT3_GEN_STOP_AT_EOS) != 0;
-  const int mode = (flags & MT3_GEN_BEAM1) ? 2 : 1;
+  const int mode = (flags & MT3_GEN_BEAM1) ? 2 : (sample && sp->temperature > kMinTemperature) ? 3 : 1;
   if (mode == 2) {      // live log-probability 0, finished score NEG_INF (t5x decoding.NEG_INF = -1e7), no finished hypothesis
     std::vector<float> init((size_t)2 * m->B);
     for (int i = 0; i < m->B; ++i) { init[2 * i] = 0.f; init[2 * i + 1] = -1.0e7f; }
@@ -1255,20 +1280,29 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
 
 extern "C" int mt3_generate(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                             int32_t* steps_run, void* stream) {
-  return generate_impl("mt3_generate", h, x, num_steps, flags, nullptr, 0, tokens_out, nullptr, nullptr, steps_run, nullptr, 0, stream);
+  return generate_impl("mt3_generate", h, x, num_steps, flags, nullptr, 0, tokens_out, nullptr, nullptr, steps_run, nullptr, 0, nullptr,
+                       stream);
 }
 
 extern "C" int mt3_generate_scored(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, int32_t* tokens_out,
                                    float* token_scores_out, float* scores_out, int32_t* steps_run, void* stream) {
   return generate_impl("mt3_generate_scored", h, x, num_steps, flags, nullptr, 0, tokens_out, token_scores_out, scores_out, steps_run,
-                       nullptr, 0, stream);
+                       nullptr, 0, nullptr, stream);
 }
 
 extern "C" int mt3_generate_prompted(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
                                      int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out,
                                      int32_t* steps_run, void* workspace, int64_t workspace_bytes, void* stream) {
   return generate_impl("mt3_generate_prompted", h, x, num_steps, flags, prompt, prompt_len, tokens_out, token_scores_out, scores_out,
-                       steps_run, workspace, workspace_bytes, stream);
+                       steps_run, workspace, workspace_bytes, nullptr, stream);
+}
+
+extern "C" int mt3_generate_sampled(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
+                                    int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out,
+                                    int32_t* steps_run, void* workspace, int64_t workspace_bytes, const mt3_sample_params* params,
+                                    void* stream) {
+  return generate_impl("mt3_generate_sampled", h, x, num_steps, flags, prompt, prompt_len, tokens_out, token_scores_out, scores_out,
+                       steps_run, workspace, workspace_bytes, params, stream);
 }
 
 extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length, int32_t target_length) {

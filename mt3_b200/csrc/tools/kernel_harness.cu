@@ -205,6 +205,17 @@ KH_API int kh_argmax_step_forced(const float* logits, int V, int B, int* tok_cur
                             pe_rows, D, y_next, n_cta, 0);
 }
 
+// sample_step_kernel (mt3_generate_sampled): B CTAs, sp DEV (mt3_sample_params); token_scores and plen may be NULL.
+// Top-k / top-p at V > kSampleMaxSortV are refused here, as mt3_generate_sampled refuses them.
+KH_API int kh_sample_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores, int out_ld,
+                          const int* plen, int* state, const mt3_sample_params* sp, int topk, float topp, const float* emb, const float* pe,
+                          int pe_rows, int D, float* y_next) {
+  MT3_REQUIRE(V <= kSampleMaxSortV || !((topk > 0 && topk < V) || (topp > 0.f && topp < 1.f)), MT3_ERR_UNSUPPORTED,
+              "kh_sample_step: top-k / top-p need V <= %d", kSampleMaxSortV);
+  return launch_sample_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next,
+                            0);
+}
+
 KH_API int kh_beam1_step_forced(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                                 int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
                                 int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next) {

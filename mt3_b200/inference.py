@@ -60,7 +60,7 @@ class InferenceModel(object):
 
     def __init__(self, checkpoint_path, model_type='mt3', *, device='cuda:0', batch_size: int = 8,
                  gin_dir: Optional[str] = None, gemm_mode: int = _lib.GEMM_TF32X3, use_graph: bool = True,
-                 kv_format: int = _lib.KV_P24, decode: str = 'greedy'):
+                 kv_format: int = _lib.KV_P24, decode: str = 'greedy', sample_params: Optional[Dict] = None):
         # Model Constants (notebook :175-185).
         if model_type == 'ismir2021':
             num_velocity_bins = 127
@@ -83,7 +83,12 @@ class InferenceModel(object):
         self.use_graph = use_graph
         self._gemm_mode = gemm_mode
         self._kv_format = kv_format
-        self.decode = decode              # 'greedy' | 'beam1' (T5X beam_search at num_decodes=1, models.py:127)
+        self.decode = decode              # 'greedy' | 'beam1' (T5X beam_search at num_decodes=1, models.py:127) | 'sample'
+        # decode='sample': Transformer.generate's temperature / topk / topp / rescale_log_probs; the seed is per call
+        self.sample_params = dict(sample_params or {})
+        unknown = set(self.sample_params) - {'temperature', 'topk', 'topp', 'rescale_log_probs'}
+        if unknown:
+            raise ValueError('sample_params takes temperature, topk, topp and rescale_log_probs; got %s' % sorted(unknown))
 
         # Build Codecs and Vocabularies (notebook :198-206).
         self.spectrogram_config = spectrograms.SpectrogramConfig()
@@ -158,23 +163,26 @@ class InferenceModel(object):
     def predict_tokens(self, batch, seed=0):
         """Predict tokens from a preprocessed batch (notebook :277-281).  batch['encoder_input_tokens']
         float32 [B, T, 512] (numpy or torch).  Returns decoded ids np.int32 [B, 1024]: id-3, -1 from
-        the first EOS on, -2 for invalid ids.  `seed` is accepted and unused: decode_rng=None (:268)."""
-        del seed
+        the first EOS on, -2 for invalid ids.  `seed` keys decode='sample' (row b draws from stream b); greedy and beam1
+        ignore it, as decode_rng=None does (:268)."""
         x = batch['encoder_input_tokens']
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(np.ascontiguousarray(x, np.float32)).to(self.device, non_blocking=True)
-        prediction = self.model.generate(x, stop_at_eos=True, use_graph=self.use_graph, decode=self.decode)
+        prediction = self.model.generate(x, stop_at_eos=True, use_graph=self.use_graph, decode=self.decode, **self._sample_kw(seed, 0))
         return self.vocabulary.decode_tf(prediction).cpu().numpy()
 
     def transcribe_segments(self, audio_segments, n_valid_frames=None, num_steps: Optional[int] = None,
-                            stop_at_eos: bool = True, decoded: bool = True, return_scores: bool = False, prompts=None):
+                            stop_at_eos: bool = True, decoded: bool = True, return_scores: bool = False, prompts=None, seed=0,
+                            segment_offset: int = 0):
         """Hot path end to end for already-cut segments: host float32 [S, inputs_length*hop] ->
         host int32 [S, 1024].  H2D copy, log-mel kernel, encoder, greedy decoder, (vocab decode),
         D2H copy; batches of `batch_size`.  This is the call bench.py's `e2e` times.
         return_scores=True returns (tokens, token_scores float32 [S, 1024], scores float32 [S]) with the same tokens: how sure
         the model was of each emitted token (its log-probability; 0 after EOS) and of each segment (Transformer.generate).
         prompts: host int [S, P], a forced start per segment (Transformer.generate's `prompt`), e.g. the tie section of
-        segment_score_targets' decoder_target_tokens: the output rows start with them and decode on from there."""
+        segment_score_targets' decoder_target_tokens: the output rows start with them and decode on from there.
+        seed (decode='sample'): segment s draws from stream segment_offset + s, so its tokens do not depend on batch_size,
+        nor on how transcribe_segments_sharded splits the segments (it passes each shard's first global index)."""
         a = audio_segments
         if isinstance(a, np.ndarray):
             a = torch.from_numpy(a)
@@ -201,7 +209,8 @@ class InferenceModel(object):
             spec = self._pad_inputs(spec)
             toks = self.model.generate(spec, num_steps=num_steps, stop_at_eos=stop_at_eos, use_graph=self.use_graph,
                                        decode=self.decode, return_scores=return_scores,
-                                       prompt=None if prompts is None else prompts[s0:s1])
+                                       prompt=None if prompts is None else prompts[s0:s1],
+                                       **self._sample_kw(seed, segment_offset + s0))
             if return_scores:
                 toks, ts, sc = toks
                 out_ts[s0:s1].copy_(ts, non_blocking=True)
@@ -235,7 +244,7 @@ class InferenceModel(object):
             nv = np.asarray(nv)[lo:hi]
         scored = kwargs.get('return_scores', False)
         if hi > lo:
-            local = self.transcribe_segments(a[lo:hi], n_valid_frames=nv, **kwargs)
+            local = self.transcribe_segments(a[lo:hi], n_valid_frames=nv, segment_offset=lo, **kwargs)
         else:
             empty = np.zeros((0, self.outputs_length), np.int32)
             local = (empty, empty.astype(np.float32), np.zeros((0,), np.float32)) if scored else empty
@@ -245,6 +254,12 @@ class InferenceModel(object):
         toks, ts, sc = (mt3_dist.gather_tokens(t.to(self.device), S).cpu().numpy()
                         for t in (torch.from_numpy(toks), torch.from_numpy(ts), torch.from_numpy(sc)[:, None]))
         return toks, ts, sc[:, 0]
+
+    def _sample_kw(self, seed, row_offset: int) -> Dict:
+        """generate's sampling arguments for a batch whose first row is segment row_offset (none unless decode='sample')"""
+        if self.decode != 'sample':
+            return {}
+        return dict(self.sample_params, seed=seed, row_offset=row_offset)
 
     def _pad_inputs(self, spec: torch.Tensor) -> torch.Tensor:
         """Feature converter (models.py:96): trim/pad the frame axis to inputs_length with 0.0."""

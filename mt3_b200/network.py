@@ -10,12 +10,31 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import math
 from typing import Dict, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib, weights as W
+
+SAMPLE_MAX_FILTER_VOCAB = 4096      # top-k / top-p sort the logits row in one CTA's shared memory (layers.cuh)
+
+
+def sample_key(seed):
+    """The 64-bit Philox key (k0, k1) of a sampling seed: an int s in [0, 2**64) gives (s >> 32, s & 0xffffffff), the two
+    words of jax.random.PRNGKey(s); two uint32 words (a PRNGKey, numpy or torch) are taken as they are."""
+    if isinstance(seed, (int, np.integer)) and not isinstance(seed, bool):
+        s = int(seed)
+        if not 0 <= s < 2 ** 64:
+            raise ValueError(f'seed must lie in [0, 2**64); got {s}')
+        return s >> 32, s & 0xffffffff
+    if isinstance(seed, torch.Tensor):
+        seed = seed.detach().cpu().numpy()
+    k = np.asarray(seed)
+    if k.shape != (2,) or k.dtype.kind not in 'iu' or (k < 0).any() or (k >= 2 ** 32).any():
+        raise ValueError(f'seed must be an int or two uint32 words; got {seed!r}')
+    return int(k[0]), int(k[1])
 
 
 @dataclasses.dataclass
@@ -248,7 +267,8 @@ class Transformer:
 
     def generate(self, encoder_input_tokens: torch.Tensor, num_steps: Optional[int] = None, stop_at_eos: bool = True,
                  use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy', return_scores: bool = False,
-                 prompt=None):
+                 prompt=None, temperature: float = 1.0, topk: int = 0, topp: float = 0.0, seed=0, row_offset: int = 0,
+                 rescale_log_probs: bool = True):
         """encode + decode from BOS=0 (models.py:121-138).  decode='greedy': argmax until EOS; decode='beam1': T5X's
         decoding.beam_search at num_decodes=1, the reference's decode_fn (models.py:127) -- they differ when EOS is one of the
         two best tokens without being decisive (tests/test_beam1.py).  Returns raw model ids int32 [B, max_decode_length],
@@ -259,11 +279,19 @@ class Transformer:
         prompt: int [B, P] (torch or numpy), T5X's prompt_with_targets: row b's non-zero prefix is forced -- the output row
         starts with it, its positions score 0, and the loop chooses from its end on.  Ids in [2, vocab_size), 0 after the
         prefix, no EOS, P <= num_steps (mt3_generate_prompted).  The prefix every row shares is prefilled by one
-        teacher-forced pass."""
-        if decode not in ('greedy', 'beam1'):
-            raise ValueError("decode must be 'greedy' or 'beam1'")
+        teacher-forced pass.
+        decode='sample': T5X's decoding.temperature_sample (mt3_generate_sampled).  Each free position draws its token from
+        softmax(logits / temperature), cut to the top `topk` ids (0: off; ties at the k-th value kept) and then to the
+        smallest most-likely set whose probability reaches `topp` (0 or 1: off).  temperature <= 1e-4 is greedy, bit for bit.
+        `seed` is an int (the key of jax.random.PRNGKey(seed)) or a key's two uint32 words; row b draws from stream
+        row_offset + b, so a row's tokens depend on (seed, row_offset + b) and its input only.  With return_scores, token
+        scores are log-probabilities under the distribution sampled from (rescale_log_probs=True, T5X's default) or under
+        the model's own softmax (False, greedy's), and the sequence score is their sum."""
+        if decode not in ('greedy', 'beam1', 'sample'):
+            raise ValueError("decode must be 'greedy', 'beam1' or 'sample'")
         x = self._check_inputs(encoder_input_tokens)
         b, t, _ = x.shape
+        sp = self._sample_params(temperature, topk, topp, seed, row_offset, rescale_log_probs, b) if decode == 'sample' else None
         steps = self.max_decode_length if num_steps is None else int(num_steps)
         if prompt is not None:
             prompt = self._check_prompt(prompt, b, steps)
@@ -271,10 +299,10 @@ class Transformer:
         if out is None:
             out = torch.empty((b, self.max_decode_length), dtype=torch.int32, device=self.device)
         flags = (_lib.GEN_STOP_AT_EOS if stop_at_eos else 0) | (_lib.GEN_USE_GRAPH if use_graph else 0) | \
-                (_lib.GEN_BEAM1 if decode == 'beam1' else 0)
+                (_lib.GEN_BEAM1 if decode == 'beam1' else 0) | (_lib.GEN_SAMPLE if sp is not None else 0)
         ran = C.c_int32(0)
-        if prompt is not None and prompt.shape[1] > 0:
-            return self._generate_prompted(x, steps, flags, prompt, out, return_scores)
+        if sp is not None or (prompt is not None and prompt.shape[1] > 0):
+            return self._generate_prompted(x, steps, flags, prompt, out, return_scores, sp)
         if not return_scores:
             with torch.cuda.device(self.device):
                 _lib.check(self._lib.mt3_generate(self._h, x.data_ptr(), steps, flags, out.data_ptr(), C.byref(ran), self._stream()))
@@ -307,16 +335,41 @@ class Transformer:
                 raise ValueError('prompt: a row has non-zero ids after its first 0 (PAD ends the prompt)')
         return p
 
-    def _generate_prompted(self, x, steps: int, flags: int, prompt: torch.Tensor, out: torch.Tensor, return_scores: bool):
+    def _sample_params(self, temperature, topk, topp, seed, row_offset, rescale_log_probs, batch: int) -> _lib.SampleParams:
+        """The host-side check of generate's sampling arguments (the library checks them again)."""
+        temperature, topp = float(temperature), float(topp)
+        if not (math.isfinite(temperature) and temperature >= 0):
+            raise ValueError(f'temperature must be finite and >= 0; got {temperature}')
+        if int(topk) != topk or not 0 <= topk < 2 ** 31:
+            raise ValueError(f'topk must be an int >= 0; got {topk!r}')
+        if not 0.0 <= topp <= 1.0:
+            raise ValueError(f'topp must lie in [0, 1]; got {topp}')
+        v = self.config.vocab_size
+        if v > SAMPLE_MAX_FILTER_VOCAB and (0 < topk < v or 0 < topp < 1):
+            raise ValueError(f'top-k / top-p need vocab_size <= {SAMPLE_MAX_FILTER_VOCAB}; this model has {v}')
+        if int(row_offset) != row_offset or not 0 <= row_offset <= 2 ** 32 - batch:
+            raise ValueError(f'row_offset must be an int in [0, 2**32 - batch]; got {row_offset!r}')
+        sp = _lib.SampleParams()
+        sp.temperature, sp.topk, sp.topp = temperature, int(topk), topp
+        sp.key[0], sp.key[1] = sample_key(seed)
+        sp.row0, sp.rescale_log_probs = int(row_offset), int(bool(rescale_log_probs))
+        return sp
+
+    def _generate_prompted(self, x, steps: int, flags: int, prompt: Optional[torch.Tensor], out: torch.Tensor, return_scores: bool,
+                           sp: Optional[_lib.SampleParams] = None):
         b, t, _ = x.shape
-        ws = self._tf_workspace(b, t, prompt.shape[1])
+        plen = 0 if prompt is None else prompt.shape[1]
+        ws = self._tf_workspace(b, t, plen) if plen else None
         token_scores = torch.empty((b, self.max_decode_length), dtype=torch.float32, device=self.device) if return_scores else None
         scores = torch.empty((b,), dtype=torch.float32, device=self.device) if return_scores else None
         ran = C.c_int32(0)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.mt3_generate_prompted(
-                self._h, x.data_ptr(), steps, flags, prompt.data_ptr(), prompt.shape[1], out.data_ptr(),
+        args = (self._h, x.data_ptr(), steps, flags, prompt.data_ptr() if plen else None, plen, out.data_ptr(),
                 None if token_scores is None else token_scores.data_ptr(), None if scores is None else scores.data_ptr(), C.byref(ran),
-                ws.data_ptr(), ws.numel(), self._stream()))
+                ws.data_ptr() if plen else None, ws.numel() if plen else 0)
+        with torch.cuda.device(self.device):
+            if sp is None:
+                _lib.check(self._lib.mt3_generate_prompted(*args, self._stream()))
+            else:
+                _lib.check(self._lib.mt3_generate_sampled(*args, C.byref(sp), self._stream()))
         self.last_steps_run = int(ran.value)
         return (out, token_scores, scores) if return_scores else out
