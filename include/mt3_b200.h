@@ -273,6 +273,27 @@ int mt3_generate_sampled(mt3_model* m, const float* x, int32_t num_steps, int32_
                          int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run, void* workspace,
                          int64_t workspace_bytes, const mt3_sample_params* params, void* stream);
 
+/* mt3_generate_sampled with an additive logit bias per sequence: which tokens the loop may emit (e.g. only some instruments).
+ *   logit_bias DEV f32, row b at logit_bias + b * bias_ld; bias_ld = 0 gives every sequence the same row, otherwise
+ *   bias_ld >= vocab_size.  Each entry is finite or -inf (-inf suppresses the id), and each row keeps at least one finite id.
+ *   Every token picker (greedy, MT3_GEN_BEAM1, MT3_GEN_SAMPLE) behaves exactly as if the model had produced
+ *     l'[b, i] = -inf where logit_bias[b, i] == -inf, else logits[b, i] + logit_bias[b, i] (one float32 add)
+ *   instead of its logits: the choice of token, the NaN rule (a NaN at a suppressed id is never emitted), EOS, and every
+ *   score.  Token scores are therefore log-probabilities under the constrained model -- greedy l'[next] - logsumexp(l');
+ *   beam1's candidates, "prefix + EOS" hypotheses and length-normalised score; sampling z = l' / temperature, its top-k /
+ *   top-p cuts and Gumbel-max over z, and l'[next] - logsumexp(l') with rescale_log_probs = 0.
+ *   Forced prompt positions are the caller's tokens even where suppressed.  A sequence whose EOS is -inf cannot finish before
+ *   num_steps.  With a bias of all zeros every output is bit-identical to an unbiased call.  mt3_decode_teacher_forced and
+ *   mt3_decode_step stay unbiased.
+ * The rows are copied into the model workspace and checked on the device before the encoder runs (one small kernel and an
+ * 8-byte copy back, which synchronises the stream): a NaN or +inf entry, a row without a finite entry, or a bias_ld that is
+ * neither 0 nor >= vocab_size returns MT3_ERR_BAD_ARG and leaves the model usable.  The biased pickers run in CUDA graphs of
+ * their own, with no extra launch per step.  With logit_bias == NULL this is mt3_generate_sampled, bit for bit. */
+int mt3_generate_biased(mt3_model* m, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt, int32_t prompt_len,
+                        int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run, void* workspace,
+                        int64_t workspace_bytes, const mt3_sample_params* params, const float* logit_bias, int64_t bias_ld,
+                        void* stream);
+
 /* GenericTokenVocabulary._decode_tf (vocabularies.py:241-271): ids DEV i32 [B, L]
  * -> out DEV i32 [B, L] with id-3, EOS-and-after = -1, invalid = -2. */
 int mt3_vocab_decode(const int32_t* ids, int32_t batch, int32_t length, int32_t num_regular_tokens, int32_t* out,

@@ -26,6 +26,7 @@ EXPORTS = [
     "mt3_workspace_bytes", "mt3_model_set_workspace", "mt3_encode", "mt3_cross_kv", "mt3_decode_step",
     "mt3_generate", "mt3_generate_scored", "mt3_vocab_decode", "mt3_dot_product_attention_f32", "mt3_debug_launch", "mt3_debug_trace_step",
     "mt3_teacher_forced_workspace_bytes", "mt3_decode_teacher_forced", "mt3_generate_prompted", "mt3_generate_sampled",
+    "mt3_generate_biased",
 ]
 
 
@@ -91,6 +92,8 @@ def load() -> C.CDLL:
     lib.mt3_generate_prompted.argtypes = [vp, f32p, i32, i32, i32p, i32, i32p, f32p, f32p, C.POINTER(i32), vp, i64, vp]
     lib.mt3_generate_sampled.argtypes = [vp, f32p, i32, i32, i32p, i32, i32p, f32p, f32p, C.POINTER(i32), vp, i64,
                                          C.POINTER(SampleParams), vp]
+    lib.mt3_generate_biased.argtypes = [vp, f32p, i32, i32, i32p, i32, i32p, f32p, f32p, C.POINTER(i32), vp, i64,
+                                        C.POINTER(SampleParams), f32p, i64, vp]
     lib.mt3_vocab_decode.argtypes = [i32p, i32, i32, i32, i32p, vp]
     lib.mt3_dot_product_attention_f32.argtypes = [f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p, vp]
     lib.mt3_debug_launch.argtypes = [vp, i32, i32, i32, vp]

@@ -269,11 +269,17 @@ inline int launch_embed(const int* tok, const float* emb, int D, int vocab, cons
 // token scores, so that one logits row gives the same bits in both: the row maximum (fmaxf, so NaN is skipped), then
 // sum expf(x - max) per thread in id order, a warp tree and the 8 warp sums in order.  A NaN in the row makes the sum, and
 // the result, NaN.  Every thread calls it (it synchronises the CTA) and every thread gets the result.  red: 8 shared floats.
+// BIAS: over the biased row biased_logit(x, bias) instead of x (mt3_generate_biased).
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, int V, float* red) {
+// The logit a token picker sees under a logit bias c: -inf where c is -inf (a suppressed id, whatever the model's logit,
+// NaN included), else one float32 add.  A zero bias gives x back bit for bit for every x but -0.0, which compares equal.
+__device__ __forceinline__ float biased_logit(float x, float c) { return c == -INFINITY ? -INFINITY : x + c; }
+
+template <bool BIAS = false>
+__device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, int V, float* red, const float* __restrict__ bias = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float mx = -INFINITY;
-  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, x[c]);
+  for (int c = tid; c < V; c += 256) mx = fmaxf(mx, BIAS ? biased_logit(x[c], bias[c]) : x[c]);
   mx = warp_max(mx);
   if (lane == 0) red[warp] = mx;
   __syncthreads();
@@ -282,7 +288,7 @@ __device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, in
   for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
   __syncthreads();
   float se = 0.f;
-  for (int c = tid; c < V; c += 256) se += expf(x[c] - mx);
+  for (int c = tid; c < V; c += 256) se += expf((BIAS ? biased_logit(x[c], bias[c]) : x[c]) - mx);
   se = warp_sum(se);
   if (lane == 0) red[warp] = se;
   __syncthreads();
@@ -304,13 +310,16 @@ __device__ __forceinline__ float block_logsumexp(const float* __restrict__ x, in
 // y_next (optional) = E[next] + PE[pos + 1], skipped at the last step, where pos + 1 = pe_rows has no PE row.
 // plen (optional, [B]): forced prompt lengths (mt3_generate_prompted).  At pos < plen[b] the sequence emits the token the
 // caller put at tokens_out[b, pos] instead of its argmax: score 0, no finish; tok_cur and y_next follow that token.
+// BIAS (argmax_step_biased_kernel): every read of the logits row is biased_logit(logits[b, i], bias[b, i]), bias [B, V]
+// (mt3_generate_biased); argmax_step_kernel is the body at BIAS = false, as it was before the bias existed.
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
-                   int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
-                   const int* __restrict__ plen, int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0,
-                   const float* __restrict__ emb,
-                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+template <bool BIAS>
+__device__ __forceinline__ void
+argmax_step_body(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
+                 int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
+                 const int* __restrict__ plen, int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0,
+                 const float* __restrict__ emb,
+                 const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next, const float* __restrict__ bias) {
   __shared__ float sv[8], slse[8];
   __shared__ int si[8], snan[8];
   __shared__ int s_next[2];
@@ -321,12 +330,13 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
   pdl_wait();
   pdl_trigger();
   const float* l = logits + (long long)b * V;
+  const float* bb = BIAS ? bias + (long long)b * V : nullptr;
   // every number beats the start (-inf, 0x7fffffff), so bi stays out of range only when the whole row is NaN, and then
   // nan_i = 0 replaces it
   float best = -INFINITY;
   int bi = 0x7fffffff, nan_i = 0x7fffffff;
   for (int i = tid; i < V; i += 256) {
-    const float v = l[i];
+    const float v = BIAS ? biased_logit(l[i], bb[i]) : l[i];
     if (v > best || (v == best && i < bi)) { best = v; bi = i; }
     if (v != v) nan_i = min(nan_i, i);
   }
@@ -339,7 +349,7 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
   nan_i = __reduce_min_sync(0xffffffffu, nan_i);
   if (lane == 0) { sv[warp] = best; si[warp] = bi; snan[warp] = nan_i; }
   __syncthreads();
-  const float lse = token_scores ? block_logsumexp(l, V, slse) : 0.f;
+  const float lse = token_scores ? block_logsumexp<BIAS>(l, V, slse, bb) : 0.f;
   if (tid == 0) {
     for (int w = 1; w < 8; ++w) {
       if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
@@ -348,7 +358,7 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
     if (nan_i != 0x7fffffff) bi = nan_i;
     const int pos = state[0];
     int nxt = bi;
-    float lp = token_scores ? l[bi] - lse : 0.f;
+    float lp = token_scores ? (BIAS ? biased_logit(l[bi], bb[bi]) : l[bi]) - lse : 0.f;
     if (pos < pl) {                       // forced: the prompt token (never EOS), so the sequence cannot finish here
       nxt = tokens_out[(long long)b * out_ld + pos];
       lp = 0.f;
@@ -396,12 +406,37 @@ argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restri
   }
 }
 
-// sequences b0 .. b0 + n_cta - 1 of a batch of B
+__global__ void __launch_bounds__(256)
+argmax_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
+                   int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
+                   const int* __restrict__ plen, int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0,
+                   const float* __restrict__ emb,
+                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+  argmax_step_body<false>(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb,
+                          pe, pe_rows, D, y_next, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
+argmax_step_biased_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur,
+                          int* __restrict__ finished, int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld,
+                          const int* __restrict__ plen, int* __restrict__ tok_out_user, int* __restrict__ state, int advance, int b0,
+                          const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next,
+                          const float* __restrict__ bias) {
+  argmax_step_body<true>(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb,
+                         pe, pe_rows, D, y_next, bias);
+}
+
+// sequences b0 .. b0 + n_cta - 1 of a batch of B; bias [B, V] or null (the unbiased kernel)
 inline int launch_argmax_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                               int out_ld, const int* plen, int* tok_out_user, int* state, int advance, int b0, const float* emb,
-                              const float* pe, int pe_rows, int D, float* y_next, int n_cta, cudaStream_t s) {
-  MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
-                               token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
+                              const float* pe, int pe_rows, int D, float* y_next, int n_cta, const float* bias, cudaStream_t s) {
+  if (bias)
+    MT3_CUDA_CHECK(launch_kernel(argmax_step_biased_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished,
+                                 tokens_out, token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next,
+                                 bias));
+  else
+    MT3_CUDA_CHECK(launch_kernel(argmax_step_kernel, dim3(n_cta), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
+                                 token_scores, out_ld, plen, tok_out_user, state, advance, b0, emb, pe, pe_rows, D, y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -434,11 +469,15 @@ __device__ __forceinline__ bool cand_better(float v, int i, float ov, int oi) {
   return !isnan(ov) && (v > ov || (v == ov && i < oi));
 }
 
-__global__ void __launch_bounds__(256)
-beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
-                  int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
-                  int* __restrict__ state, float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
-                  const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+// BIAS (beam1_step_biased_kernel): every read of the logits row is biased_logit(logits[b, i], bias[b, i]), as in
+// argmax_step_body.
+template <bool BIAS>
+__device__ __forceinline__ void
+beam1_step_body(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
+                int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                int* __restrict__ state, float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
+                const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next,
+                const float* __restrict__ bias) {
   __shared__ float s1v[8], s2v[8], smx[8], ssum[8];
   __shared__ int s1i[8], s2i[8];
   __shared__ int s_next[2];
@@ -447,11 +486,12 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
   pdl_wait();
   pdl_trigger();
   const float* l = logits + (long long)b * V;
+  const float* bb = BIAS ? bias + (long long)b * V : nullptr;
   // best and second-best NON-EOS candidates (value, id), and the running maximum over everything for the log-sum-exp
   float v1 = -INFINITY, v2 = -INFINITY, mx = -INFINITY;
   int i1 = 0x7fffffff, i2 = 0x7fffffff;
   for (int i = tid; i < V; i += 256) {
-    const float v = l[i];
+    const float v = BIAS ? biased_logit(l[i], bb[i]) : l[i];
     mx = fmaxf(mx, v);
     if (i == 1) continue;                        // EOS (vocabularies.py:157-159) is handled separately
     if (cand_better(v, i, v1, i1)) { v2 = v1; i2 = i1; v1 = v; i1 = i; }
@@ -473,7 +513,7 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
 #pragma unroll
   for (int w = 1; w < 8; ++w) gmx = fmaxf(gmx, smx[w]);
   float se = 0.f;
-  for (int i = tid; i < V; i += 256) se += expf(l[i] - gmx);
+  for (int i = tid; i < V; i += 256) se += expf((BIAS ? biased_logit(l[i], bb[i]) : l[i]) - gmx);
   se = warp_sum(se);
   if (lane == 0) ssum[warp] = se;
   __syncthreads();
@@ -489,7 +529,7 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
     float tot = 0.f;
     for (int w = 0; w < 8; ++w) tot += ssum[w];
     const float lse = gmx + logf(tot);
-    const float veos = l[1];
+    const float veos = BIAS ? biased_logit(l[1], bb[1]) : l[1];
     const int pos = state[0];
     const float live_prev = beam_f[2 * b];
     float fin_score = beam_f[2 * b + 1];
@@ -538,11 +578,38 @@ beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restric
   }
 }
 
+__global__ void __launch_bounds__(256)
+beam1_step_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
+                  int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                  int* __restrict__ state, float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i, float alpha, int max_len,
+                  const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+  beam1_step_body<false>(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha,
+                         max_len, emb, pe, pe_rows, D, y_next, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
+beam1_step_biased_kernel(const float* __restrict__ logits, int V, int B, int* __restrict__ tok_cur, int* __restrict__ finished,
+                         int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                         int* __restrict__ state, float* __restrict__ beam_f, float* __restrict__ fin_lp_eos, int* __restrict__ beam_i,
+                         float alpha, int max_len, const float* __restrict__ emb, const float* __restrict__ pe, int pe_rows, int D,
+                         float* __restrict__ y_next, const float* __restrict__ bias) {
+  beam1_step_body<true>(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha,
+                        max_len, emb, pe, pe_rows, D, y_next, bias);
+}
+
+// bias [B, V] or null (the unbiased kernel)
 inline int launch_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                              int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
-                             int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next, cudaStream_t s) {
-  MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
-                               token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D, y_next));
+                             int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next, const float* bias,
+                             cudaStream_t s) {
+  if (bias)
+    MT3_CUDA_CHECK(launch_kernel(beam1_step_biased_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
+                                 token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D,
+                                 y_next, bias));
+  else
+    MT3_CUDA_CHECK(launch_kernel(beam1_step_kernel, dim3(B), dim3(256), 0, s, false, logits, V, B, tok_cur, finished, tokens_out,
+                                 token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i, alpha, max_len, emb, pe, pe_rows, D,
+                                 y_next));
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }
@@ -629,12 +696,15 @@ __device__ __forceinline__ uint32_t z_order_desc(float z) {
   return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
 }
 
-__global__ void __launch_bounds__(256)
-sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, int* __restrict__ tok_cur, int* __restrict__ finished,
-                   int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
-                   int* __restrict__ state, const mt3_sample_params* __restrict__ sp, const float* __restrict__ emb,
-                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
+// BIAS (sample_step_biased_kernel): every read of the logits row is biased_logit(logits[b, i], bias[b, i]), as in
+// argmax_step_body: z = biased logits / temperature, and the unrescaled scores are taken over the biased row.
+template <bool BIAS>
+__device__ __forceinline__ void
+sample_step_body(const float* __restrict__ logits, int V, int B, int nsort, int* __restrict__ tok_cur, int* __restrict__ finished,
+                 int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                 int* __restrict__ state, const mt3_sample_params* __restrict__ sp, const float* __restrict__ emb,
+                 const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next, const float* __restrict__ bias,
+                 unsigned char* smem_raw) {
   unsigned long long* skey = reinterpret_cast<unsigned long long*>(smem_raw);   // [nsort] (z order << 32 | id)
   float* z = reinterpret_cast<float*>(smem_raw + (size_t)nsort * 8);              // [V]
   __shared__ float sv[8], slse[8], sscan[8];
@@ -650,11 +720,12 @@ sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, in
   pdl_wait();
   pdl_trigger();
   const float* l = logits + (long long)b * V;
+  const float* bb = BIAS ? bias + (long long)b * V : nullptr;
   // read by every thread before its CTA arrives at the counter (the barriers below), so before the last CTA advances it
   const int pos = state[0];
   int nan_i = 0x7fffffff;
   for (int i = tid; i < V; i += 256) {
-    const float v = l[i];
+    const float v = BIAS ? biased_logit(l[i], bb[i]) : l[i];
     z[i] = v / temp;
     if (v != v) nan_i = min(nan_i, i);
   }
@@ -756,13 +827,19 @@ sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, in
   }
   if (lane == 0) { sv[warp] = best; si[warp] = bi; }
   __syncthreads();
-  const float lse = (token_scores && !has_nan) ? block_logsumexp(rescale ? z : l, V, slse) : 0.f;
+  float lse = 0.f;
+  if constexpr (BIAS) {
+    if (token_scores && !has_nan) lse = rescale ? block_logsumexp(z, V, slse) : block_logsumexp<true>(l, V, slse, bb);
+  } else {
+    lse = (token_scores && !has_nan) ? block_logsumexp(rescale ? z : l, V, slse) : 0.f;
+  }
   if (tid == 0) {
     for (int w = 1; w < 8; ++w)
       if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
     int nxt = has_nan ? nan_i : bi;
     float lp = 0.f;
-    if (token_scores) lp = has_nan ? __int_as_float(0x7fffffff) : (rescale ? z[nxt] : l[nxt]) - lse;
+    if (token_scores)
+      lp = has_nan ? __int_as_float(0x7fffffff) : (rescale ? z[nxt] : (BIAS ? biased_logit(l[nxt], bb[nxt]) : l[nxt])) - lse;
     if (pos < pl) {                       // forced: the prompt token (never EOS), so the sequence cannot finish here
       nxt = tokens_out[(long long)b * out_ld + pos];
       lp = 0.f;
@@ -800,15 +877,42 @@ sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, in
   }
 }
 
-// every sequence of a batch of B; sp DEV.  Top-k / top-p at V > kSampleMaxSortV are refused by the caller, which knows sp.
+__global__ void __launch_bounds__(256)
+sample_step_kernel(const float* __restrict__ logits, int V, int B, int nsort, int* __restrict__ tok_cur, int* __restrict__ finished,
+                   int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                   int* __restrict__ state, const mt3_sample_params* __restrict__ sp, const float* __restrict__ emb,
+                   const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  sample_step_body<false>(logits, V, B, nsort, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D,
+                          y_next, nullptr, smem_raw);
+}
+
+__global__ void __launch_bounds__(256)
+sample_step_biased_kernel(const float* __restrict__ logits, int V, int B, int nsort, int* __restrict__ tok_cur, int* __restrict__ finished,
+                          int* __restrict__ tokens_out, float* __restrict__ token_scores, int out_ld, const int* __restrict__ plen,
+                          int* __restrict__ state, const mt3_sample_params* __restrict__ sp, const float* __restrict__ emb,
+                          const float* __restrict__ pe, int pe_rows, int D, float* __restrict__ y_next, const float* __restrict__ bias) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  sample_step_body<true>(logits, V, B, nsort, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D,
+                         y_next, bias, smem_raw);
+}
+
+// every sequence of a batch of B; sp DEV; bias [B, V] or null (the unbiased kernel).  Top-k / top-p at V > kSampleMaxSortV are
+// refused by the caller, which knows sp.
 inline int launch_sample_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                               int out_ld, const int* plen, int* state, const mt3_sample_params* sp, const float* emb, const float* pe,
-                              int pe_rows, int D, float* y_next, cudaStream_t s) {
+                              int pe_rows, int D, float* y_next, const float* bias, cudaStream_t s) {
   const size_t smem = sample_step_smem(V);
   MT3_REQUIRE(smem <= (size_t)kSampleMaxSmem, MT3_ERR_UNSUPPORTED, "sampling: vocabulary %d too large for one CTA's row", V);
-  MT3_TRY(set_max_dynamic_smem<sample_step_kernel>(kSampleMaxSmem));
-  MT3_CUDA_CHECK(launch_kernel(sample_step_kernel, dim3(B), dim3(256), smem, s, false, logits, V, B, sample_sort_n(V), tok_cur, finished,
-                               tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next));
+  if (bias) {
+    MT3_TRY(set_max_dynamic_smem<sample_step_biased_kernel>(kSampleMaxSmem));
+    MT3_CUDA_CHECK(launch_kernel(sample_step_biased_kernel, dim3(B), dim3(256), smem, s, false, logits, V, B, sample_sort_n(V), tok_cur,
+                                 finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next, bias));
+  } else {
+    MT3_TRY(set_max_dynamic_smem<sample_step_kernel>(kSampleMaxSmem));
+    MT3_CUDA_CHECK(launch_kernel(sample_step_kernel, dim3(B), dim3(256), smem, s, false, logits, V, B, sample_sort_n(V), tok_cur, finished,
+                                 tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next));
+  }
   MT3_LAUNCH_CHECK();
   return MT3_OK;
 }

@@ -127,6 +127,7 @@ struct WsBuffers {
   int* prompt_info = nullptr;     // {P = shortest prompt, 1 + first invalid row or 0} of prompt_scan_kernel
   int* pf_tok = nullptr;          // [2][B, L] decoder inputs and key-validity targets of the prefill pass
   mt3_sample_params* sample = nullptr;   // the sampling picker's parameters (MT3_GEN_SAMPLE), written once per generate
+  float* bias = nullptr;          // [B, V] the token pickers' logit bias (mt3_generate_biased), written once per biased generate
   float* dpartial = nullptr;      // split-K scratch of the non-cluster decode GEMM
   int* dcounters = nullptr;       // [dec_tiles()]
 };
@@ -555,8 +556,9 @@ static int dec_layer_mlp(Model* m, const DecBranch& b, int l, cudaStream_t s) {
 // loop_step: a step of mt3_generate's loop -- the decoder input m->dy was already written (by dec_embed before the first
 // step, by the previous step's argmax kernel afterwards), and this step's argmax kernel writes the next one.
 // scored: the token picker also writes each emitted token's log-probability to m->tok_scores (mt3_generate_scored).
+// biased: the loop's token picker reads its logits through the logit bias m->bias (mt3_generate_biased).
 static int decode_step_impl(Model* m, const int* tok_in, float* logits, int greedy, int* tok_user, int use_finished,
-                            int* tokens_ws, cudaStream_t s, bool loop_step = false, bool scored = false) {
+                            int* tokens_ws, cudaStream_t s, bool loop_step = false, bool scored = false, bool biased = false) {
   if (!loop_step) MT3_TRY(dec_embed(m, tok_in, s));
   DecBranch b{m->dy, false};
   for (int l = 0; l < m->Ld; ++l) {
@@ -570,16 +572,17 @@ static int decode_step_impl(Model* m, const int* tok_in, float* logits, int gree
                    kv_stage_for(m, 0, 1), dec_chain(m, true, false)));
   float* y_next = loop_step ? m->dy : nullptr;
   float* tok_scores = scored ? m->tok_scores : nullptr;
+  const float* bias = loop_step && biased ? m->bias : nullptr;
   if (greedy == 2) {        // T5X beam_search bookkeeping at num_decodes = 1 (generate loop only)
     MT3_TRY(launch_beam1_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->beam_f,
-                              m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, kPeRows, m->D, y_next, s));
+                              m->fin_lp_eos, m->beam_i, 0.6f, m->L, m->emb, m->pe, kPeRows, m->D, y_next, bias, s));
   } else if (greedy == 3) { // T5X temperature_sample's pick (generate loop only), parameters in the workspace
     MT3_TRY(launch_sample_step(logits, m->V, m->B, m->tok_cur, m->finished, tokens_ws, tok_scores, m->L, m->plen, m->state, m->sample,
-                               m->emb, m->pe, kPeRows, m->D, y_next, s));
+                               m->emb, m->pe, kPeRows, m->D, y_next, bias, s));
   } else if (greedy) {
     MT3_TRY(launch_argmax_step(logits, m->V, m->B, use_finished ? m->tok_cur : nullptr, use_finished ? m->finished : nullptr, tokens_ws,
                                tok_scores, m->L, loop_step ? m->plen : nullptr, tok_user, m->state, 1, 0, m->emb, m->pe, kPeRows, m->D,
-                               y_next, m->B, s));
+                               y_next, m->B, bias, s));
   } else {
     MT3_CUDA_CHECK(launch_kernel(advance_pos_kernel, dim3(1), dim3(1), 0, s, false, m->state));
     MT3_LAUNCH_CHECK();
@@ -610,9 +613,10 @@ static void select_graph(Model* m, int mode = 1) {
 
 // mode: 1 greedy, 2 beam-size-1 search, 3 sampling; nsteps consecutive decode steps per graph (the position lives on the device, so a
 // graph of 16 steps is the single-step graph 16 times over: one graph launch and its ~3 us of inter-launch latency per 16 steps);
-// scored: the token pickers write token scores (a graph of its own, so that the unscored graphs do no extra work)
-static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
-  const int key = mode | (scored ? 4 : 0) | (nsteps << 8);
+// scored: the token pickers write token scores (a graph of its own, so that the unscored graphs do no extra work);
+// biased: the token pickers read the logit bias (a graph of its own, so that the unbiased graphs keep their kernels)
+static int ensure_graph(Model* m, int mode, int nsteps, bool scored, bool biased) {
+  const int key = mode | (scored ? 4 : 0) | (biased ? 8 : 0) | (nsteps << 8);
   if (m->graph_mode != key) select_graph(m, key);
   if (m->graph_exec) return MT3_OK;
   if (!m->cap_stream) MT3_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
@@ -620,7 +624,7 @@ static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
   MT3_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
   int r = MT3_OK;
   for (int i = 0; i < nsteps && r == MT3_OK; ++i)
-    r = decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, m->cap_stream, true, scored);
+    r = decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, m->cap_stream, true, scored, biased);
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaStreamEndCapture(m->cap_stream, &g);
   if (r != MT3_OK) {
@@ -632,10 +636,10 @@ static int ensure_graph(Model* m, int mode, int nsteps, bool scored) {
   m->graph_kernels = g_launch_count.load() - before;
   g_launch_count.fetch_sub(m->graph_kernels);   // capture does not execute
   MT3_CUDA_CHECK(cudaGraphInstantiate(&m->graph_exec, m->graph, 0));
-  // bound the cache: forget the graphs of other (workspace, B, T) bindings.  The current binding's stay: it has at most 12
-  // (3 modes x scored or not x 1 or 16 steps), and a caller may still hold one of them (mt3_generate_scored keeps the
-  // 16-step graph while it makes sure of the single-step one).
-  if (m->graphs.size() >= 16) {
+  // bound the cache: forget the graphs of other (workspace, B, T) bindings.  The current binding's stay: it has at most 24
+  // (3 modes x scored or not x biased or not x 1 or 16 steps), and a caller may still hold one of them (mt3_generate_scored
+  // keeps the 16-step graph while it makes sure of the single-step one).
+  if (m->graphs.size() >= 32) {
     for (auto it = m->graphs.begin(); it != m->graphs.end();) {
       if (std::get<0>(it->first) != (const void*)m->ws || std::get<1>(it->first) != m->B || std::get<2>(it->first) != m->T) {
         cudaGraphExecDestroy(it->second.e);
@@ -1039,6 +1043,7 @@ static int carve_workspace(const Model* m, Carve& c, int B, int T, WsBuffers* w)
   w->prompt_info = c.take<int>(2);
   w->pf_tok = c.take<int>(2 * B * L);
   w->sample = c.take<mt3_sample_params>(1);
+  w->bias = c.take((int64_t)B * m->V);
   return MT3_OK;
 }
 
@@ -1127,6 +1132,31 @@ __global__ void __launch_bounds__(256) prompt_scan_kernel(const int* __restrict_
   if (threadIdx.x == 0) { info[0] = s_min; info[1] = s_bad < B ? s_bad + 1 : 0; }
 }
 
+// Logit bias rows (mt3_generate_biased), one warp per row: dst[b, :] = bias[b * ld, ...] ([B, V]; ld = 0 repeats one row).
+// A row is valid when every entry is finite or -inf and at least one is finite.  info[1] holds 0 or prompt_scan_kernel's
+// code on entry; a 0 becomes -(1 + the first invalid row), so one 8-byte copy reports both checks.
+__global__ void __launch_bounds__(1024) bias_load_kernel(const float* __restrict__ bias, long long ld, int B, int V,
+                                                         float* __restrict__ dst, int* __restrict__ info) {
+  __shared__ int s_bad;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_bad = B;
+  __syncthreads();
+  for (int b = warp; b < B; b += 32) {
+    const float* row = bias + b * ld;
+    bool bad = false, finite = false;
+    for (int j = lane; j < V; j += 32) {
+      const float v = row[j];
+      bad |= !(v < INFINITY);             // NaN or +inf
+      finite |= v > -INFINITY && v < INFINITY;
+      dst[(long long)b * V + j] = v;
+    }
+    const bool row_bad = __any_sync(0xffffffffu, bad) || !__any_sync(0xffffffffu, finite);
+    if (row_bad && lane == 0) atomicMin(&s_bad, b);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_bad < B && info[1] == 0) info[1] = -(s_bad + 1);
+}
+
 // The prefill pass's inputs over the shared prefix of P positions: decoder inputs BOS, prompt[:, 0 .. P-2] and targets
 // prompt[:, 0 .. P-1] (all non-zero: every key < P is valid), both [B, P]; and the loop's state after it: position P, next
 // decoder input prompt[:, P-1].
@@ -1151,11 +1181,13 @@ constexpr int kPrefillMinP = 20;
 // Temperatures at or below this pick greedily (T5X's MIN_TEMPERATURE): MT3_GEN_SAMPLE then runs the greedy loop unchanged.
 constexpr float kMinTemperature = 1e-4f;
 
-// mt3_generate, mt3_generate_scored, mt3_generate_prompted and mt3_generate_sampled; `name` is the entry point the caller used,
-// for its error messages.  prompt_len == 0: no prompt (prompt and workspace unused).  sp: HOST, read with MT3_GEN_SAMPLE only.
+// mt3_generate, mt3_generate_scored, mt3_generate_prompted, mt3_generate_sampled and mt3_generate_biased; `name` is the entry
+// point the caller used, for its error messages.  prompt_len == 0: no prompt (prompt and workspace unused).  sp: HOST, read
+// with MT3_GEN_SAMPLE only.  bias: DEV or null (no bias), rows bias_ld apart.
 static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
                          int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out, int32_t* steps_run,
-                         void* workspace, int64_t workspace_bytes, const mt3_sample_params* sp, void* stream) {
+                         void* workspace, int64_t workspace_bytes, const mt3_sample_params* sp, void* stream,
+                         const float* bias = nullptr, int64_t bias_ld = 0) {
   MT3_REQUIRE(h && x && tokens_out, MT3_ERR_BAD_ARG, "%s: null argument", name);
   Model* m = reinterpret_cast<Model*>(h);
   MT3_NEED_WS(m);
@@ -1179,6 +1211,9 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
               num_steps);
   MT3_REQUIRE(prompt_len == 0 || prompt, MT3_ERR_BAD_ARG, "%s: prompt is NULL with prompt_len %d", name, prompt_len);
   if (prompt_len > 0) MT3_TRY(check_tf_workspace(m, name, workspace, workspace_bytes, m->B, m->T, prompt_len));
+  const bool biased = bias != nullptr;
+  MT3_REQUIRE(!biased || bias_ld == 0 || bias_ld >= m->V, MT3_ERR_BAD_ARG, "%s: bias_ld %lld is neither 0 nor >= vocab_size %d", name,
+              (long long)bias_ld, m->V);
   cudaStream_t s = (cudaStream_t)stream;
   MT3_CUDA_CHECK(cudaMemsetAsync(m->tokens, 0, (size_t)m->B * m->L * sizeof(int), s));
   MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
@@ -1188,13 +1223,23 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
     MT3_CUDA_CHECK(cudaStreamSynchronize(s));        // `sp` is the caller's pageable memory
   }
   int P = 0;                                    // prompt prefix every row shares
-  if (prompt_len > 0) {
-    prompt_scan_kernel<<<1, 256, 0, s>>>(prompt, m->B, prompt_len, m->V, m->plen, m->tokens, m->L, m->prompt_info);
-    MT3_LAUNCH_CHECK();
+  if (prompt_len > 0 || biased) {
+    if (prompt_len > 0) {
+      prompt_scan_kernel<<<1, 256, 0, s>>>(prompt, m->B, prompt_len, m->V, m->plen, m->tokens, m->L, m->prompt_info);
+      MT3_LAUNCH_CHECK();
+    } else {
+      MT3_CUDA_CHECK(cudaMemsetAsync(m->prompt_info, 0, 2 * sizeof(int), s));
+    }
+    if (biased) {     // the picker reads the bias from the workspace, so one graph per (mode, scored, steps) serves every bias
+      bias_load_kernel<<<1, 1024, 0, s>>>(bias, (long long)bias_ld, m->B, m->V, m->bias, m->prompt_info);
+      MT3_LAUNCH_CHECK();
+    }
     MT3_CUDA_CHECK(cudaMemcpyAsync(m->h_flag + 2, m->prompt_info, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
     MT3_CUDA_CHECK(cudaStreamSynchronize(s));
     if (m->h_flag[3]) {
       MT3_CUDA_CHECK(cudaMemsetAsync(m->plen, 0, (size_t)m->B * sizeof(int), s));
+      if (m->h_flag[3] < 0)
+        return fail(MT3_ERR_BAD_ARG, "%s: logit_bias row %d holds a NaN or +inf, or no finite entry", name, -m->h_flag[3] - 1);
       return fail(MT3_ERR_BAD_ARG, "%s: prompt row %d is not a prefix of ids in [2, %d) followed by zeros", name, m->h_flag[3] - 1, m->V);
     }
     P = m->h_flag[2];
@@ -1232,11 +1277,11 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
   uint64_t k1 = 0, kN = 0;
   if (use_graph) {
     if (num_steps - start >= kBlock) {
-      MT3_TRY(ensure_graph(m, mode, kBlock, scored));
+      MT3_TRY(ensure_graph(m, mode, kBlock, scored, biased));
       gN = m->graph_exec; kN = m->graph_kernels;
     }
     if ((num_steps - start) % kBlock != 0) {
-      MT3_TRY(ensure_graph(m, mode, 1, scored));
+      MT3_TRY(ensure_graph(m, mode, 1, scored, biased));
       g1 = m->graph_exec; k1 = m->graph_kernels;
     }
   }
@@ -1253,7 +1298,7 @@ static int generate_impl(const char* name, mt3_model* h, const float* x, int32_t
       MT3_CUDA_CHECK(cudaGraphLaunch(g1, s));
       count_launch(k1);
     } else {
-      MT3_TRY(decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, s, true, scored));
+      MT3_TRY(decode_step_impl(m, m->tok_cur, m->dlogits, mode, nullptr, 1, m->tokens, s, true, scored, biased));
     }
     step += n;
     ran += n;
@@ -1303,6 +1348,14 @@ extern "C" int mt3_generate_sampled(mt3_model* h, const float* x, int32_t num_st
                                     void* stream) {
   return generate_impl("mt3_generate_sampled", h, x, num_steps, flags, prompt, prompt_len, tokens_out, token_scores_out, scores_out,
                        steps_run, workspace, workspace_bytes, params, stream);
+}
+
+extern "C" int mt3_generate_biased(mt3_model* h, const float* x, int32_t num_steps, int32_t flags, const int32_t* prompt,
+                                   int32_t prompt_len, int32_t* tokens_out, float* token_scores_out, float* scores_out,
+                                   int32_t* steps_run, void* workspace, int64_t workspace_bytes, const mt3_sample_params* params,
+                                   const float* logit_bias, int64_t bias_ld, void* stream) {
+  return generate_impl("mt3_generate_biased", h, x, num_steps, flags, prompt, prompt_len, tokens_out, token_scores_out, scores_out,
+                       steps_run, workspace, workspace_bytes, params, stream, logit_bias, bias_ld);
 }
 
 extern "C" int64_t mt3_teacher_forced_workspace_bytes(const mt3_model* h, int32_t batch, int32_t input_length, int32_t target_length) {

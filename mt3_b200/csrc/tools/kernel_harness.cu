@@ -166,14 +166,14 @@ KH_API int kh_argmax_step(const float* logits, int V, int B, int* tok_cur, int* 
                           int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows, int D, float* y_next,
                           int n_cta) {
   return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, nullptr, tok_user, state, advance, b0, emb, pe,
-                            pe_rows, D, y_next, n_cta, 0);
+                            pe_rows, D, y_next, n_cta, nullptr, 0);
 }
 
 KH_API int kh_beam1_step(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, int out_ld, int* state,
                          float* beam_f, int* beam_i, float alpha, int max_len, const float* emb, const float* pe, int pe_rows, int D,
                          float* y_next) {
   return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, nullptr, out_ld, nullptr, state, beam_f, nullptr, beam_i, alpha,
-                           max_len, emb, pe, pe_rows, D, y_next, 0);
+                           max_len, emb, pe, pe_rows, D, y_next, nullptr, 0);
 }
 
 KH_API int kh_beam1_finalize(int* tokens, int B, int L, int steps, const int* beam_i) {
@@ -186,14 +186,14 @@ KH_API int kh_argmax_step_scored(const float* logits, int V, int B, int* tok_cur
                                  int out_ld, int* tok_user, int* state, int advance, int b0, const float* emb, const float* pe, int pe_rows,
                                  int D, float* y_next, int n_cta) {
   return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, nullptr, tok_user, state, advance, b0, emb,
-                            pe, pe_rows, D, y_next, n_cta, 0);
+                            pe, pe_rows, D, y_next, n_cta, nullptr, 0);
 }
 
 KH_API int kh_beam1_step_scored(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                                 int out_ld, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha, int max_len,
                                 const float* emb, const float* pe, int pe_rows, int D, float* y_next) {
   return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, nullptr, state, beam_f, fin_lp_eos, beam_i,
-                           alpha, max_len, emb, pe, pe_rows, D, y_next, 0);
+                           alpha, max_len, emb, pe, pe_rows, D, y_next, nullptr, 0);
 }
 
 // The forced forms (mt3_generate_prompted): plen [B] prompt lengths; at pos < plen[b] the kernels emit tokens_out[b, pos]
@@ -202,7 +202,7 @@ KH_API int kh_argmax_step_forced(const float* logits, int V, int B, int* tok_cur
                                  int out_ld, const int* plen, int* tok_user, int* state, int advance, int b0, const float* emb,
                                  const float* pe, int pe_rows, int D, float* y_next, int n_cta) {
   return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, tok_user, state, advance, b0, emb, pe,
-                            pe_rows, D, y_next, n_cta, 0);
+                            pe_rows, D, y_next, n_cta, nullptr, 0);
 }
 
 // sample_step_kernel (mt3_generate_sampled): B CTAs, sp DEV (mt3_sample_params); token_scores and plen may be NULL.
@@ -213,14 +213,42 @@ KH_API int kh_sample_step(const float* logits, int V, int B, int* tok_cur, int* 
   MT3_REQUIRE(V <= kSampleMaxSortV || !((topk > 0 && topk < V) || (topp > 0.f && topp < 1.f)), MT3_ERR_UNSUPPORTED,
               "kh_sample_step: top-k / top-p need V <= %d", kSampleMaxSortV);
   return launch_sample_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next,
-                            0);
+                            nullptr, 0);
 }
 
 KH_API int kh_beam1_step_forced(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
                                 int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
                                 int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next) {
   return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i,
-                           alpha, max_len, emb, pe, pe_rows, D, y_next, 0);
+                           alpha, max_len, emb, pe, pe_rows, D, y_next, nullptr, 0);
+}
+
+// The biased pickers (mt3_generate_biased): the forced forms above with bias [B, V] (row stride V), which the picker reads
+// through biased_logit.  token_scores, fin_lp_eos and plen may be NULL; bias may not (NULL launches the unbiased kernel).
+KH_API int kh_argmax_step_biased(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                 int out_ld, const int* plen, int* tok_user, int* state, int advance, int b0, const float* emb,
+                                 const float* pe, int pe_rows, int D, float* y_next, int n_cta, const float* bias) {
+  MT3_REQUIRE(bias, MT3_ERR_BAD_ARG, "kh_argmax_step_biased: null bias");
+  return launch_argmax_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, tok_user, state, advance, b0, emb, pe,
+                            pe_rows, D, y_next, n_cta, bias, 0);
+}
+
+KH_API int kh_beam1_step_biased(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                int out_ld, const int* plen, int* state, float* beam_f, float* fin_lp_eos, int* beam_i, float alpha,
+                                int max_len, const float* emb, const float* pe, int pe_rows, int D, float* y_next, const float* bias) {
+  MT3_REQUIRE(bias, MT3_ERR_BAD_ARG, "kh_beam1_step_biased: null bias");
+  return launch_beam1_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, beam_f, fin_lp_eos, beam_i,
+                           alpha, max_len, emb, pe, pe_rows, D, y_next, bias, 0);
+}
+
+KH_API int kh_sample_step_biased(const float* logits, int V, int B, int* tok_cur, int* finished, int* tokens_out, float* token_scores,
+                                 int out_ld, const int* plen, int* state, const mt3_sample_params* sp, int topk, float topp, const float* emb,
+                                 const float* pe, int pe_rows, int D, float* y_next, const float* bias) {
+  MT3_REQUIRE(bias, MT3_ERR_BAD_ARG, "kh_sample_step_biased: null bias");
+  MT3_REQUIRE(V <= kSampleMaxSortV || !((topk > 0 && topk < V) || (topp > 0.f && topp < 1.f)), MT3_ERR_UNSUPPORTED,
+              "kh_sample_step_biased: top-k / top-p need V <= %d", kSampleMaxSortV);
+  return launch_sample_step(logits, V, B, tok_cur, finished, tokens_out, token_scores, out_ld, plen, state, sp, emb, pe, pe_rows, D, y_next,
+                            bias, 0);
 }
 
 KH_API int kh_beam1_finalize_scored(int* tokens, int B, int L, int steps, const int* beam_i, float* token_scores, const float* beam_f,

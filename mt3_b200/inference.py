@@ -22,7 +22,7 @@ A "dataset" here is a list of example dicts.  Divergences from the notebook, rec
 from __future__ import annotations
 
 import os
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -58,9 +58,12 @@ def segment_score_targets(note_sequence, codec, vocabulary, frame_times, inputs_
 class InferenceModel(object):
     """Wrapper of the H100 model for music transcription."""
 
+    logit_bias = None     # float32 [vocab_size] of programs= / drums=, or None (no restriction)
+
     def __init__(self, checkpoint_path, model_type='mt3', *, device='cuda:0', batch_size: int = 8,
                  gin_dir: Optional[str] = None, gemm_mode: int = _lib.GEMM_TF32X3, use_graph: bool = True,
-                 kv_format: int = _lib.KV_P24, decode: str = 'greedy', sample_params: Optional[Dict] = None):
+                 kv_format: int = _lib.KV_P24, decode: str = 'greedy', sample_params: Optional[Dict] = None,
+                 programs: Optional[Sequence[int]] = None, drums: bool = True):
         # Model Constants (notebook :175-185).
         if model_type == 'ismir2021':
             num_velocity_bins = 127
@@ -98,6 +101,10 @@ class InferenceModel(object):
         self.output_features = {'inputs': {'dtype': 'float32', 'rank': 2}, 'targets': {'vocabulary': self.vocabulary}}
 
         self._parse_gin(gin_files)
+        # restrict the instruments: the decoder may emit only the program events of `programs` (None: all) and no drum
+        # events when drums=False -- a logit bias row (vocabularies.program_logit_bias) that every decode mode applies
+        if programs is not None or not drums:
+            self.logit_bias = vocabularies.program_logit_bias(self.codec, self._model_config().vocab_size, programs, drums)
         self.model = None
         self.restore_from_checkpoint(checkpoint_path)
 
@@ -168,7 +175,8 @@ class InferenceModel(object):
         x = batch['encoder_input_tokens']
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(np.ascontiguousarray(x, np.float32)).to(self.device, non_blocking=True)
-        prediction = self.model.generate(x, stop_at_eos=True, use_graph=self.use_graph, decode=self.decode, **self._sample_kw(seed, 0))
+        prediction = self.model.generate(x, stop_at_eos=True, use_graph=self.use_graph, decode=self.decode, **self._sample_kw(seed, 0),
+                                         **self._bias_kw())
         return self.vocabulary.decode_tf(prediction).cpu().numpy()
 
     def transcribe_segments(self, audio_segments, n_valid_frames=None, num_steps: Optional[int] = None,
@@ -210,7 +218,7 @@ class InferenceModel(object):
             toks = self.model.generate(spec, num_steps=num_steps, stop_at_eos=stop_at_eos, use_graph=self.use_graph,
                                        decode=self.decode, return_scores=return_scores,
                                        prompt=None if prompts is None else prompts[s0:s1],
-                                       **self._sample_kw(seed, segment_offset + s0))
+                                       **self._sample_kw(seed, segment_offset + s0), **self._bias_kw())
             if return_scores:
                 toks, ts, sc = toks
                 out_ts[s0:s1].copy_(ts, non_blocking=True)
@@ -260,6 +268,10 @@ class InferenceModel(object):
         if self.decode != 'sample':
             return {}
         return dict(self.sample_params, seed=seed, row_offset=row_offset)
+
+    def _bias_kw(self) -> Dict:
+        """generate's logit_bias argument (none unless programs= or drums=False restrict the instruments)"""
+        return {} if self.logit_bias is None else {'logit_bias': self.logit_bias}
 
     def _pad_inputs(self, spec: torch.Tensor) -> torch.Tensor:
         """Feature converter (models.py:96): trim/pad the frame axis to inputs_length with 0.0."""

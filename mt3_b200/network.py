@@ -268,7 +268,7 @@ class Transformer:
     def generate(self, encoder_input_tokens: torch.Tensor, num_steps: Optional[int] = None, stop_at_eos: bool = True,
                  use_graph: bool = True, out: Optional[torch.Tensor] = None, decode: str = 'greedy', return_scores: bool = False,
                  prompt=None, temperature: float = 1.0, topk: int = 0, topp: float = 0.0, seed=0, row_offset: int = 0,
-                 rescale_log_probs: bool = True):
+                 rescale_log_probs: bool = True, logit_bias=None):
         """encode + decode from BOS=0 (models.py:121-138).  decode='greedy': argmax until EOS; decode='beam1': T5X's
         decoding.beam_search at num_decodes=1, the reference's decode_fn (models.py:127) -- they differ when EOS is one of the
         two best tokens without being decisive (tests/test_beam1.py).  Returns raw model ids int32 [B, max_decode_length],
@@ -286,7 +286,12 @@ class Transformer:
         `seed` is an int (the key of jax.random.PRNGKey(seed)) or a key's two uint32 words; row b draws from stream
         row_offset + b, so a row's tokens depend on (seed, row_offset + b) and its input only.  With return_scores, token
         scores are log-probabilities under the distribution sampled from (rescale_log_probs=True, T5X's default) or under
-        the model's own softmax (False, greedy's), and the sequence score is their sum."""
+        the model's own softmax (False, greedy's), and the sequence score is their sum.
+        logit_bias: float32 [V] (one row for every sequence) or [B, V] (numpy or torch), added to the logits of every free
+        position before the token is picked, in every decode mode (mt3_generate_biased): -inf suppresses an id, whatever the
+        model's logit.  Entries must be finite or -inf, with at least one finite entry per row.  Token and sequence scores
+        are then log-probabilities under the biased logits; prompt tokens are forced even where suppressed, and a row whose
+        EOS is -inf runs to num_steps.  score() and decode() stay unbiased."""
         if decode not in ('greedy', 'beam1', 'sample'):
             raise ValueError("decode must be 'greedy', 'beam1' or 'sample'")
         x = self._check_inputs(encoder_input_tokens)
@@ -295,14 +300,15 @@ class Transformer:
         steps = self.max_decode_length if num_steps is None else int(num_steps)
         if prompt is not None:
             prompt = self._check_prompt(prompt, b, steps)
+        bias = None if logit_bias is None else self._check_logit_bias(logit_bias, b)
         self._bind(b, t)
         if out is None:
             out = torch.empty((b, self.max_decode_length), dtype=torch.int32, device=self.device)
         flags = (_lib.GEN_STOP_AT_EOS if stop_at_eos else 0) | (_lib.GEN_USE_GRAPH if use_graph else 0) | \
                 (_lib.GEN_BEAM1 if decode == 'beam1' else 0) | (_lib.GEN_SAMPLE if sp is not None else 0)
         ran = C.c_int32(0)
-        if sp is not None or (prompt is not None and prompt.shape[1] > 0):
-            return self._generate_prompted(x, steps, flags, prompt, out, return_scores, sp)
+        if sp is not None or bias is not None or (prompt is not None and prompt.shape[1] > 0):
+            return self._generate_prompted(x, steps, flags, prompt, out, return_scores, sp, bias)
         if not return_scores:
             with torch.cuda.device(self.device):
                 _lib.check(self._lib.mt3_generate(self._h, x.data_ptr(), steps, flags, out.data_ptr(), C.byref(ran), self._stream()))
@@ -335,6 +341,22 @@ class Transformer:
                 raise ValueError('prompt: a row has non-zero ids after its first 0 (PAD ends the prompt)')
         return p
 
+    def _check_logit_bias(self, logit_bias, batch: int) -> torch.Tensor:
+        """The host-side check of a generate logit bias (the library checks it again on the device): float32 [V] or [B, V] on
+        the device, contiguous (its row stride is then 0 or V)."""
+        t = torch.from_numpy(logit_bias) if isinstance(logit_bias, np.ndarray) else logit_bias
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+            raise ValueError('logit_bias must be a float32 numpy array or torch tensor')
+        v = self.config.vocab_size
+        if tuple(t.shape) not in ((v,), (batch, v)):
+            raise ValueError(f'logit_bias must have shape ({v},) or ({batch}, {v}); got {tuple(t.shape)}')
+        rows = t.detach().reshape(-1, v).cpu()
+        if bool(torch.isnan(rows).any()) or bool((rows == math.inf).any()):
+            raise ValueError('logit_bias: entries must be finite or -inf (no NaN, no +inf)')
+        if not bool(torch.isfinite(rows).any(1).all()):
+            raise ValueError('logit_bias: every row must keep at least one finite entry')
+        return t.to(device=self.device).contiguous()
+
     def _sample_params(self, temperature, topk, topp, seed, row_offset, rescale_log_probs, batch: int) -> _lib.SampleParams:
         """The host-side check of generate's sampling arguments (the library checks them again)."""
         temperature, topp = float(temperature), float(topp)
@@ -356,7 +378,7 @@ class Transformer:
         return sp
 
     def _generate_prompted(self, x, steps: int, flags: int, prompt: Optional[torch.Tensor], out: torch.Tensor, return_scores: bool,
-                           sp: Optional[_lib.SampleParams] = None):
+                           sp: Optional[_lib.SampleParams] = None, bias: Optional[torch.Tensor] = None):
         b, t, _ = x.shape
         plen = 0 if prompt is None else prompt.shape[1]
         ws = self._tf_workspace(b, t, plen) if plen else None
@@ -367,7 +389,10 @@ class Transformer:
                 None if token_scores is None else token_scores.data_ptr(), None if scores is None else scores.data_ptr(), C.byref(ran),
                 ws.data_ptr() if plen else None, ws.numel() if plen else 0)
         with torch.cuda.device(self.device):
-            if sp is None:
+            if bias is not None:
+                _lib.check(self._lib.mt3_generate_biased(*args, None if sp is None else C.byref(sp), bias.data_ptr(),
+                                                         0 if bias.dim() == 1 else bias.shape[1], self._stream()))
+            elif sp is None:
                 _lib.check(self._lib.mt3_generate_prompted(*args, self._stream()))
             else:
                 _lib.check(self._lib.mt3_generate_sampled(*args, C.byref(sp), self._stream()))

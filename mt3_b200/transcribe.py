@@ -3,11 +3,13 @@ colab/music_transcription_with_transformers.ipynb) as one command.
 
     python -m mt3_b200.transcribe input.wav output.mid --checkpoint CKPT [--model mt3|ismir2021]
            [--batch-size 64] [--decode greedy|beam1] [--jsonl notes.jsonl] [--device cuda:0]
+           [--programs 0,1,...] [--no-drums]
 
 CKPT is what InferenceModel.restore_from_checkpoint takes: a .npz keyed by the Flax tree paths, a T5X checkpoint
 directory (mt3_b200.checkpoints), or 'synthetic[:SEED]' for random weights (plumbing runs only -- the published
 checkpoints at gs://mt3/checkpoints are unreachable offline).  Launched under torch.distributed.run the segments are
-sharded over the GPUs (InferenceModel.predict_segments) and rank 0 writes the files.
+sharded over the GPUs (InferenceModel.predict_segments) and rank 0 writes the files.  --programs and --no-drums restrict
+the instruments the decoder may emit (InferenceModel's programs= and drums=), e.g. `--programs 0 --no-drums` for solo piano.
 """
 from __future__ import annotations
 
@@ -30,7 +32,21 @@ def _parser() -> argparse.ArgumentParser:
     ap.add_argument('--decode', default='greedy', choices=['greedy', 'beam1'])
     ap.add_argument('--device', default=None, help="default: cuda:LOCAL_RANK")
     ap.add_argument('--jsonl', default=None, help='also write the notes as one JSON line (the T5X-infer style record)')
+    ap.add_argument('--programs', type=_programs, default=None,
+                    help='comma-separated MIDI programs (0-127) the decoder may emit; default: every program')
+    ap.add_argument('--no-drums', dest='drums', action='store_false', help='the decoder emits no drum events')
     return ap
+
+
+def _programs(text: str) -> List[int]:
+    try:
+        programs = [int(p) for p in text.split(',')]
+    except ValueError:
+        raise argparse.ArgumentTypeError('expected comma-separated integers, got %r' % text)
+    bad = [p for p in programs if not 0 <= p <= 127]
+    if bad:
+        raise argparse.ArgumentTypeError('MIDI programs lie in 0..127; got %s' % bad)
+    return programs
 
 
 def main(argv: Optional[List[str]] = None) -> int:
@@ -53,7 +69,8 @@ def main(argv: Optional[List[str]] = None) -> int:
     if world > 1 and not torch.distributed.is_initialized():
         torch.distributed.init_process_group('nccl', device_id=torch.device(device))
     rank, _ = mt3_dist.world()
-    model = inference.InferenceModel(args.checkpoint, args.model, device=device, batch_size=args.batch_size, decode=args.decode)
+    model = inference.InferenceModel(args.checkpoint, args.model, device=device, batch_size=args.batch_size, decode=args.decode,
+                                     programs=args.programs, drums=args.drums)
     est_ns = model(audio)
     if rank == 0:
         note_decoding.note_sequence_to_midi_file(est_ns, args.midi)

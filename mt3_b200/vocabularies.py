@@ -32,6 +32,8 @@ MIN_MIDI_PITCH, MAX_MIDI_PITCH = 0, 127
 MIN_MIDI_PROGRAM, MAX_MIDI_PROGRAM = 0, 127
 MAX_MIDI_VELOCITY = 127
 
+NUM_SPECIAL_TOKENS = 3     # 0=PAD, 1=EOS, 2=UNK: model id = codec index + 3
+
 
 @dataclasses.dataclass
 class VocabularyConfig:
@@ -112,7 +114,7 @@ class GenericTokenVocabulary:
     """Vocabulary with pass-through encoding of tokens (vocabularies.py:148-277)."""
 
     def __init__(self, regular_ids: int, extra_ids: int = 0):
-        self._num_special_tokens = 3     # 0=PAD, 1=EOS, 2=UNK
+        self._num_special_tokens = NUM_SPECIAL_TOKENS
         self._num_regular_tokens = regular_ids
         self.extra_ids = extra_ids
 
@@ -191,6 +193,29 @@ class GenericTokenVocabulary:
 
 def vocabulary_from_codec(codec: event_codec.Codec) -> GenericTokenVocabulary:
     return GenericTokenVocabulary(codec.num_classes, extra_ids=DEFAULT_EXTRA_IDS)
+
+
+def program_logit_bias(codec: event_codec.Codec, vocab_size: int, programs: Optional[Sequence[int]] = None,
+                       drums: bool = True) -> np.ndarray:
+    """A logit bias float32 [vocab_size] for Transformer.generate that restricts the instruments: 0 everywhere except -inf at
+    the model id (codec index + the vocabulary's 3 special ids) of every `program` event whose MIDI program is not in
+    `programs` (None: every program allowed), and of the whole `drum` range when drums=False."""
+    if vocab_size < codec.num_classes + NUM_SPECIAL_TOKENS:
+        raise ValueError(f'vocab_size {vocab_size} is smaller than the codec\'s {codec.num_classes} ids + {NUM_SPECIAL_TOKENS}')
+    bias = np.zeros(vocab_size, np.float32)
+    if programs is not None:
+        programs = [int(p) for p in programs]
+        bad = [p for p in programs if not MIN_MIDI_PROGRAM <= p <= MAX_MIDI_PROGRAM]
+        if bad:
+            raise ValueError(f'programs must lie in [{MIN_MIDI_PROGRAM}, {MAX_MIDI_PROGRAM}]; got {bad}')
+        lo, hi = codec.event_type_range('program')
+        keep = np.zeros(hi - lo + 1, bool)
+        keep[np.asarray(programs, np.int64) - MIN_MIDI_PROGRAM] = True
+        bias[lo + NUM_SPECIAL_TOKENS:hi + 1 + NUM_SPECIAL_TOKENS][~keep] = -np.inf
+    if not drums:
+        lo, hi = codec.event_type_range('drum')
+        bias[lo + NUM_SPECIAL_TOKENS:hi + 1 + NUM_SPECIAL_TOKENS] = -np.inf
+    return bias
 
 
 def num_embeddings(vocabulary: GenericTokenVocabulary) -> int:
